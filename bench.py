@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the Selftok hot path on B200 (BASELINE.json metric).
+"""bench.py — headline benchmark of the Selftok hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU arithmetic on the host cores
@@ -13,7 +13,7 @@ checkpoint of the real architecture (no weights are obtainable offline).
 Printed JSON (rank 0, one line): metric/value/unit/... per the driver contract, plus
   e2e          the same metric through the host-buffer C-ABI entry points (pinned host -> device copies of latents,
                tokens and noise and the device -> host reads of tokens and latents inside the timed region)
-  roofline     tcgen05 GEMM class (dominant kernel): algorithmic FLOPs / summed CUDA-event time of its launches in one
+  roofline     tensor-core GEMM class (dominant kernel): algorithmic FLOPs / summed CUDA-event time of its launches in one
                profiled step, against MEASURED_PEAKS.json's sustained bf16 GEMM rate
   cpu_baseline oracle port of the reference arithmetic (torch fp32 on the host cores) on a bounded sample
   extra        (N = 1 only) sub-records for the other BASELINE configs, each measured in this run:
@@ -45,6 +45,7 @@ METRIC = "images/sec encode+50-step decode, 256x256/512-tok"
 UNIT = "images/s"
 BATCH = 64
 DECODE_STEPS = 50
+FFMA_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12      # H100 SXM fp32 FFMA, data-sheet boost clock
 
 
 def peaks():
@@ -53,7 +54,7 @@ def peaks():
         d = json.load(open(p))
         return dict(tflops=float(d["bf16_tflops_sustained"]), tflops_burst=float(d["bf16_tflops"]),
                     hbm=float(d["hbm_gbs"]), source="measured (MEASURED_PEAKS.json, sustained bf16 cuBLAS)")
-    return dict(tflops=1400.0, tflops_burst=1590.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    return dict(tflops=989.0, tflops_burst=989.0, hbm=3350.0, source="H100 SXM data sheet (dense bf16, HBM3; 700 W card)")
 
 
 def other_class_rooflines(prof, B, precision, pk):
@@ -73,7 +74,7 @@ def other_class_rooflines(prof, B, precision, pk):
     if "attention" in prof and prof["attention"][0] > 0:
         ach = attn_flops / (prof["attention"][0] / 1000.0) / 1e12
         out["attention"] = {"bound": "tensor", "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"],
-                            "note": "head dim 64: latency-chain bound, see profiles/r2_attention_investigation.md"}
+                            "note": "head dim 64"}
     if "ln_modulate" in prof and prof["ln_modulate"][0] > 0:
         ach = ln_bytes / (prof["ln_modulate"][0] / 1000.0) / 1e9
         out["ln_modulate"] = {"bound": "hbm", "achieved": ach, "peak": pk["hbm"], "unit": "GB/s", "frac": ach / pk["hbm"],
@@ -81,9 +82,9 @@ def other_class_rooflines(prof, B, precision, pk):
     if "linear_f32" in prof and prof["linear_f32"][0] > 0:
         enc_flops = 65.6e9 * B                                       # DESIGN.md section 4: encoder GEMMs per image
         ach = enc_flops / (prof["linear_f32"][0] / 1000.0) / 1e12
-        peak = 148 * 128 * 2 * 1.965e9 / 1e12
+        peak = FFMA_PEAK_TFLOPS
         out["linear_f32"] = {"bound": "fp32 FFMA", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-                             "note": "Q-Former encoder, fp32 for bit-exact ids; peak = 148 SMs x 128 lanes x 2 x 1.965 GHz (nominal)"}
+                             "note": "Q-Former encoder, fp32 for bit-exact ids; peak = 132 SMs x 128 lanes x 2 x 1.98 GHz (data-sheet boost)"}
     return out
 
 
@@ -127,19 +128,8 @@ class ClockSampler:
                 "power_w_max": max(pw) if pw else None, "samples": len(sm), "reasons": reasons}
 
 
-def gemm_traffic():
-    """DRAM bytes per tcgen05 GEMM launch: NOT measured by this run (ncu cannot run inside a timed bench) -- read from the
-    committed extract of the round's `ncu --set full` capture of one MMDiT layer (profiles/extract_ncu.py)."""
-    for name in ("r2_gemm_traffic.json", "r1_gemm_traffic.json"):
-        p = os.path.join(REPO, "profiles", name)
-        if os.path.exists(p):
-            d = json.load(open(p))
-            return {"bytes_per_launch": float(d["bytes_per_launch"]), "source": f"profiles/{name}: " + d["source"]}
-    return {"bytes_per_launch": None, "source": "no committed ncu extract"}
-
-
 def gemm_flops_per_step(B: int) -> float:
-    """Algorithmic (single-product, masked-effective) FLOPs of the tcgen05 GEMM launches of one 50-step decode:
+    """Algorithmic (single-product, masked-effective) FLOPs of the tensor-core GEMM launches of one 50-step decode:
     per layer and stream qkv 2*M*D*3D, proj 2*M*D*D, fc1+fc2 16*M*D*D; the last layer's context stream is qkv only."""
     d = C.FULL
     tb = S.make_tables(d.K, d.stages, d.k_per_stage, DECODE_STEPS)
@@ -244,6 +234,17 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
+def dump_outputs(out_dir, arrays):
+    """Write each output of the last timed step as <out_dir>/<name>.npy: token ids as float64 (exact below 2^53), the
+    decoded latents as float32.  The inputs are index-hashed, so two builds run with the same arguments can be compared
+    output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64 if a.dtype.kind in "iu" else np.float32))
+
+
 def run_extras(args, eng, dev, x0, noise, timed):
     """Sub-records for BASELINE configs 2 and 4 and the fp32-faithful mode (see the module docstring).  `eng` is the
     headline engine (still alive); every other engine is created here and closed before the next one."""
@@ -262,7 +263,7 @@ def run_extras(args, eng, dev, x0, noise, timed):
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     ts = []
     for _ in range(13):
-        flush.zero_()                                         # L2 flushed between iterations (256 MiB > 126 MB)
+        flush.zero_()                                         # L2 flushed between iterations (256 MiB > 50 MB)
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -274,7 +275,7 @@ def run_extras(args, eng, dev, x0, noise, timed):
     R = B * d.K
     vq_bytes = R * d.enc_qdim * 4 + d.codebook_size * d.code_dim * 4 + d.code_dim * d.enc_qdim * 4 + R * 8 + R * d.code_dim * 4
     vq_flops = 2.0 * R * d.codebook_size * d.code_dim + 2.0 * R * d.enc_qdim * d.code_dim
-    ffma_peak = 148 * 128 * 2 * 1.965e9 / 1e12
+    ffma_peak = FFMA_PEAK_TFLOPS
     out["config2_encode_only"] = {
         "workload": f"batch={B} 256x256 encode only (16-block Q-Former + fused VQ -> 512 tokens)", "value": B * 5 / (ms / 1000.0), "unit": UNIT,
         "ms_per_batch": ms / 5,
@@ -336,7 +337,7 @@ def run_extras(args, eng, dev, x0, noise, timed):
         z = noise * 0.5
         dec.decode(z)
         msv, _ = timed(lambda: dec.decode(z, norm_ip=True) is None, 3)
-        out["vae_decode"] = {"workload": f"batch={B} SD3 VAE decoder, 32x32x16 latents -> 256x256 pixels (split-bf16 tcgen05 implicit-GEMM convs)",
+        out["vae_decode"] = {"workload": f"batch={B} SD3 VAE decoder, 32x32x16 latents -> 256x256 pixels (split-bf16 wgmma implicit-GEMM convs)",
                              "value": B * 3 / (msv / 1000.0), "unit": UNIT, "ms_per_batch": msv / 3, "algorithmic_tflop_per_batch": 0.622 * B}
         img = synth.synth_tensor("bench.images", (B, 3, 256, 256), "emb", 0.5, device=dev)
         dec.encode(img)
@@ -406,12 +407,14 @@ def run_gpu(args):
     tok_h = torch.empty(B, d.K, dtype=torch.int64).pin_memory()
     out_h = torch.empty_like(noise_h).pin_memory()
 
+    last = {}                                       # what the timed path handed back in its latest step
+
     def step_device():
         tok = eng.encode(x0)
         n = eng.last_launch_count
         if world > 1:
             gather_tokens(tok, B * world)           # the path's only exchange: [B,512] int64 per rank over NVLink
-        eng.decode(tok, noise)
+        last["tokens"], last["latents"] = tok, eng.decode(tok, noise)
         return n + eng.last_launch_count
 
     def step_host():
@@ -449,6 +452,8 @@ def run_gpu(args):
         sampler.start()
     ms, launches = timed(step_device, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     value = B * world * args.steps / (ms / 1000.0)
     # ---- end to end through the host-buffer entry points
     step_host()
@@ -469,22 +474,18 @@ def run_gpu(args):
         eng.set_profile(False)
         eng.set_use_graph(True)
         pk = peaks()
-        traffic = gemm_traffic()
         total_ms = sum(v[0] for v in prof.values())
-        if "gemm_tcgen05" in prof:
-            g_ms, g_n = prof["gemm_tcgen05"]
+        if "gemm_tc" in prof:
+            g_ms, g_n = prof["gemm_tc"]
             flops = gemm_flops_per_step(B)
             ach = flops / (g_ms / 1000.0) / 1e12
-            roof = {"bound": "tensor", "kernel": "gemm_tc2_kernel (tcgen05 cta_group::2 kind::f16, %s)" % args.precision,
+            roof = {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma, two-CTA clusters, %s)" % args.precision,
                     "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"],
-                    "traffic": traffic["bytes_per_launch"] if B == BATCH else None, "traffic_unit": "bytes/launch",
-                    "traffic_source": traffic["source"],
                     "timed_in": "a separate graph-off pass of the same step with CUDA events around every launch (the timed region replays "
                                 "one CUDA graph; class shares of the two agree within 1 %)",
                     "peak_source": pk["source"], "launches": g_n, "avg_launch_ms": g_ms / g_n,
                     "algorithmic_flops_per_launch": flops / g_n, "share_of_step": g_ms / total_ms,
-                    "note": "FLOPs counted once per product (the bf16x3 split passes are overhead, not useful FLOPs); the peak is the bf16 cuBLAS "
-                            "figure -- IEEE-half operands draw more power per MMA, the same GEMMs on bf16 operands run 4.8 % faster at the 1 kW cap"}
+                    "note": "FLOPs counted once per product (the bf16x3 split passes are overhead, not useful FLOPs)"}
         class_roof = other_class_rooflines(prof, B, args.precision, pk)
     # ---- the other BASELINE configs, measured in the same run (N = 1 only; each engine is built, timed and released)
     extra = None
@@ -501,14 +502,14 @@ def run_gpu(args):
         eff, dense = S.decode_flops_per_image(d.K, d.stages, d.k_per_stage, DECODE_STEPS, d.dit_depth, d.n_img)
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": {"bf16x3": "bf16x3 (split-bf16 tcgen05, fp32 accumulate; encoder/VQ fp32)",
-                          "fp16": "fp16 (IEEE-half operands on tcgen05, fp32 accumulate; encoder/VQ/tables fp32)",
-                          "bf16": "bf16 (tcgen05, fp32 accumulate; encoder/VQ fp32)", "fp32": "f32"}[args.precision],
+                "dtype": {"bf16x3": "bf16x3 (split-bf16 wgmma, fp32 accumulate; encoder/VQ fp32)",
+                          "fp16": "fp16 (IEEE-half operands on wgmma, fp32 accumulate; encoder/VQ/tables fp32)",
+                          "bf16": "bf16 (wgmma, fp32 accumulate; encoder/VQ fp32)", "fp32": "f32"}[args.precision],
                 "data": "synthetic",
                 "config": {"workload": f"batch={B}/GPU 256x256 encode + 50-step diffusion decode (512 tokens, no VAE/renderer)",
                            "batch_per_gpu": B, "global_batch": B * world, "decode_steps": DECODE_STEPS, "precision": args.precision,
                            "parallelism": f"dp{world} (images sharded, weights replicated, 1 NCCL all-gather of tokens/step)",
-                           "l2": "working set >> L2 (126 MB): %.1f GB of 16-bit weight planes + ~3 GB of activations streamed per DiT step"
+                           "l2": "working set >> L2 (50 MB): %.1f GB of 16-bit weight planes + ~3 GB of activations streamed per DiT step"
                                  % (4.17 * (2 if args.precision == "bf16x3" else 1)),
                            "algorithmic_tflop_per_image": eff / 1e12},
                 "e2e": {"value": e2e, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -532,6 +533,7 @@ def main():
     ap.add_argument("--batch", type=int, default=BATCH)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extra", action="store_true", help="skip the sub-records of the other BASELINE configs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's token ids and latents to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

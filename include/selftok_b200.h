@@ -1,5 +1,5 @@
 /*
- * selftok_b200.h — C ABI of the B200-native SelftokTokenizer encode / decode hot path.
+ * selftok_b200.h — C ABI of the H100-native (sm_90a) SelftokTokenizer encode / decode hot path.
  *
  * The reference (selftok-team/SelftokTokenizer) is pure Python; the boundary it exposes for this path is the
  * class API of mimogpt/infer/SelftokPipeline.py (SelftokPipeline.encoding :210-225, .decoding :227-294,
@@ -51,16 +51,16 @@ typedef enum selftok_status {
   SELFTOK_ERR_STATE = -3,         /* call order violated (e.g. decode before finalize)             */
   SELFTOK_ERR_MISSING_TENSOR = -4,/* finalize: a checkpoint key the path needs was never loaded    */
   SELFTOK_ERR_CUDA = -5,          /* a CUDA runtime / driver call failed; see selftok_last_error() */
-  SELFTOK_ERR_NO_DEVICE = -6      /* no sm_100 device visible — there is no CPU fallback            */
+  SELFTOK_ERR_NO_DEVICE = -6      /* no sm_90 device visible — there is no CPU fallback             */
 } selftok_status;
 
 /* GEMM arithmetic of the decoder (MMDiT / renderer).  The encoder and VQ always run fp32 FFMA (token ids must
  * be bit-stable; SURVEY 7 hard part 2). */
 typedef enum selftok_precision {
   SELFTOK_PREC_FP32_SIMT = 0,     /* fp32 FFMA GEMMs + fp32 attention (bring-up / bisecting reference)       */
-  SELFTOK_PREC_BF16X3 = 1,        /* tcgen05 kind::f16: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, fp32 accumulate   */
-  SELFTOK_PREC_BF16 = 2,          /* tcgen05 kind::f16 single pass (bf16 operands, fp32 accumulate)          */
-  SELFTOK_PREC_FP16 = 3           /* tcgen05 kind::f16 single pass (IEEE half operands, fp32 accumulate)     */
+  SELFTOK_PREC_BF16X3 = 1,        /* wgmma: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, fp32 accumulate             */
+  SELFTOK_PREC_BF16 = 2,          /* wgmma single pass (bf16 operands, fp32 accumulate)                    */
+  SELFTOK_PREC_FP16 = 3           /* wgmma single pass (IEEE half operands, fp32 accumulate)               */
 } selftok_precision;
 
 /* Flat view of cfg.tokenizer.params (configs/res256/256-eval.yml:48-105) after the reference's registries
@@ -85,7 +85,7 @@ enum { SELFTOK_F32 = 0, SELFTOK_I64 = 1 };
 int selftok_create(const selftok_config_t* cfg, selftok_handle_t* out);
 int selftok_destroy(selftok_handle_t h);
 const char* selftok_last_error(void);
-/* ABI / build identification: "selftok_b200 <abi> sm_100a <build flags>" */
+/* ABI / build identification: "selftok_b200 <abi> sm_90a <build flags>" */
 const char* selftok_version(void);
 
 /* ---- weights: one call per checkpoint key, names exactly as in the reference state dict ------------------
@@ -192,7 +192,7 @@ int selftok_set_use_graph(selftok_handle_t h, int enable);
 
 /* Per-kernel-class device timing: with profiling on (and graphs off) every launch of a hot-path call is bracketed
  * by CUDA events on its stream.  selftok_get_profile synchronises, writes the summed milliseconds and launch counts
- * of the 8 classes (0 tcgen05 GEMM, 1 attention, 2 LayerNorm+modulate, 3 fp32 FFMA linear, 4 VQ, 5 other) and resets. */
+ * of the 8 classes (0 tensor-core GEMM, 1 attention, 2 LayerNorm+modulate, 3 fp32 FFMA linear, 4 VQ, 5 other) and resets. */
 int selftok_set_profile(selftok_handle_t h, int enable);
 int selftok_get_profile(selftok_handle_t h, double* ms_out /*[8]*/, int64_t* count_out /*[8]*/);
 
@@ -200,11 +200,12 @@ int selftok_get_profile(selftok_handle_t h, double* ms_out /*[8]*/, int64_t* cou
 /* y[M,N] = act(A[M,K] W[N,K]^T + bias) (+ epilogue), fp32 FFMA.  act: 0 none, 1 gelu-tanh, 2 silu. */
 int selftok_k_linear_f32(const float* A_dev, const float* W_dev, const float* bias_dev, float* out_dev,
                          int64_t M, int N, int K, int act, void* stream);
-/* Same product on the tcgen05 path: A/W given as fp32, converted to 16-bit planes internally
+/* Same product on the tensor-core (wgmma) path: A/W given as fp32, converted to 16-bit planes internally
  * (nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass). */
 int selftok_k_linear_tc(const float* A_dev, const float* W_dev, const float* bias_dev, float* out_dev,
                         int64_t M, int N, int K, int nsplit, void* stream);
-/* Process-wide choice of the tcgen05 GEMM variant: 2 = cta_group::2 SM-pair kernel (default), 1 = single-CTA kernel. */
+/* Process-wide choice of the GEMM variant: 2 = two-CTA clusters sharing the weight tile by TMA multicast (default),
+ * 1 = one CTA per tile. */
 int selftok_k_set_gemm_ctas(int n);
 /* out = LN(x) * (1 + scale[m % period]) + shift[m % period], rows of D; eps 1e-6, no affine. */
 int selftok_k_ln_mod_f32(const float* x_dev, const float* shift_dev, const float* scale_dev, int64_t ld_mod,
@@ -216,8 +217,7 @@ int selftok_k_attention_f32(const float* q_dev, int64_t q_ld, const float* k1_de
                             float* out_dev, int64_t out_ld, int B, int Sq, int H, int hd, void* stream);
 /* Tensor-core (bf16x3 / bf16) attention over a packed qkv buffer [B,S,3,H,64]; ctx_rows = number of leading rows
  * whose queries may only see the first `ctx_keys` keys (renderer rule; pass 0 for plain dense attention).
- * nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass (mma.sync kernel); 10 / 11: the tcgen05 + TMEM kernel
- * with IEEE half / bf16 operands. */
+ * nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass. */
 int selftok_k_attention_tc(const float* qkv_dev, float* out_dev, int B, int S, int H, int nsplit,
                            int ctx_rows, int ctx_keys, void* stream);
 

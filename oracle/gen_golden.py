@@ -183,7 +183,7 @@ def gen_pixels_tiny():
 
 def gen_pixels_full():
     """Full geometry, B = 1: reference latents of tests/golden/full_decode.npz and full_renderer.npz through the
-    full-size (ch = 128) reference SDVAE -> [1,3,256,256] pixels in [0,1]."""
+    full-size (ch = 128) reference SDVAE -> [1,3,256,256] pixels in [0,1] (full_pixels.npz, full_renderer_pixels.npz)."""
     vae = ref_vae(128)
     g = np.load(os.path.join(GOLD, "full_decode.npz"))
     gr = np.load(os.path.join(GOLD, "full_renderer.npz"))
@@ -191,7 +191,8 @@ def gen_pixels_full():
     px = ref_pixels(vae, torch.from_numpy(g["pred_x0"]))
     pr = ref_pixels(vae, torch.from_numpy(gr["pred_x0"]))
     print(f"SDVAE decode of 2 images: {time.time() - t0:.1f}s; in-range fraction {float(((px > 0) & (px < 1)).float().mean()):.3f}")
-    save("full_pixels", pixels=px, renderer_pixels=pr)
+    save("full_pixels", pixels=px)                      # one image per file: each stays under 1 MB
+    save("full_renderer_pixels", pixels=pr)
 
 
 def save(name, **arrs):
@@ -367,6 +368,38 @@ def gen_tiny_datasize():
     save("tiny_ds96", tokens=tokens, margin=margin, noise=noise, pred_x0=pred_x0)
 
 
+def gen_tiny_live():
+    """The reference's own encoder on the TINY geometry (synthetic checkpoint, latents "live.x0") and the key / shape list
+    of its state dict: what test_live_reference_agrees_if_mounted compares the restatement with."""
+    dims = C.TINY
+    ref_loader.import_reference()
+    sd = synth.synth_state_dict(dims)
+    enc_name, dit_name = ref_loader.register_geometry(dims, "tinylive")
+    pipe = ref_loader.build_reference_pipeline(ref_loader.dims_to_cfg(dims, enc_name, dit_name), sd)
+    ref_sd = pipe.model.state_dict()
+    names = sorted(ref_sd)
+    x0 = synth.synth_tensor("live.x0", (2, 16, 8, 8), "emb", 1.0)
+    with torch.no_grad():
+        outs_q, tokens = pipe.model.encoder(x0, d=None)
+    save("tiny_live", tokens=tokens, outs_q=outs_q, sd_keys=np.array(names),
+         sd_shapes=np.array(["x".join(str(n) for n in ref_sd[k].shape) for k in names]))
+
+
+def gen_boundary_helpers():
+    """NormalizeToTensor, norm_ip and SD3LatentFormat of the reference (SelftokPipeline.py:85-97,135-137;
+    sd3/sd3_impls.py:133-144) on fixed inputs."""
+    ref_loader.import_reference()
+    from mimogpt.infer import SelftokPipeline as SP
+    from mimogpt.models.selftok.sd3.sd3_impls import SD3LatentFormat as RefFmt
+    img = np.random.RandomState(0).randint(0, 256, size=(24, 40, 3)).astype(np.uint8)
+    x = torch.tensor([-3.0, -1.0, 0.0, 0.5, 1.0, 2.0])
+    y = x.clone()
+    SP.norm_ip(y, -1, 1)
+    lat = torch.randn(2, 16, 4, 4, generator=torch.Generator().manual_seed(0))
+    save("boundary_helpers", img=img, normalized=SP.NormalizeToTensor()(img), x=x, norm_ip=y, lat=lat,
+         lat_in=RefFmt().process_in(lat), lat_out=RefFmt().process_out(lat))
+
+
 if __name__ == "__main__":
     what = sys.argv[1:] or ["tiny"]
     pipe = None
@@ -401,5 +434,9 @@ if __name__ == "__main__":
             gen_pixels_tiny()
         elif w == "full_pixels":
             gen_pixels_full()
+        elif w == "tiny_live":
+            gen_tiny_live()
+        elif w == "boundary_helpers":
+            gen_boundary_helpers()
         else:
             raise SystemExit(f"unknown target {w}")

@@ -1,4 +1,4 @@
-"""selftoktokenizer_b200 — B200-native (sm_100a) implementation of the SelftokTokenizer encode / decode hot path.
+"""selftoktokenizer_b200 — H100-native (sm_90a) implementation of the SelftokTokenizer encode / decode hot path.
 
 Public surface mirrors mimogpt/infer/SelftokPipeline.py: `SelftokPipeline`, `NormalizeToTensor`,
 `parse_args_from_yaml`.  All arithmetic on the path runs in hand-written CUDA behind the C-ABI declared

@@ -1,6 +1,6 @@
 """ctypes binding of include/selftok_b200.h (libselftok_b200.so) — the only way Python reaches the kernels.
 
-There is deliberately no fallback: if the library is missing or no sm_100 GPU is visible, construction raises
+There is deliberately no fallback: if the library is missing or no sm_90 GPU is visible, construction raises
 (`SelftokError`).  PyTorch appears here only as the owner of device memory (`tensor.data_ptr()`) and of the
 current stream handle.
 """
@@ -412,7 +412,7 @@ class Engine:
     def set_use_graph(self, enable: bool) -> None:
         check(self.lib.selftok_set_use_graph(self.h, int(enable)))
 
-    PROFILE_CLASSES = ("gemm_tcgen05", "attention", "ln_modulate", "linear_f32", "vq", "other", "_6", "_7")
+    PROFILE_CLASSES = ("gemm_tc", "attention", "ln_modulate", "linear_f32", "vq", "other", "_6", "_7")
 
     def set_profile(self, enable: bool) -> None:
         check(self.lib.selftok_set_profile(self.h, int(enable)))

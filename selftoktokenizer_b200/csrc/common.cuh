@@ -1,4 +1,4 @@
-// Shared host/device helpers for the selftok_b200 kernels (sm_100a only).
+// Shared host/device helpers for the selftok_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -61,54 +61,22 @@ __device__ __forceinline__ float gelu_tanh_fast(float x) {
   const float u = k0 * (x + k1 * x * x * x);
   return __fdividef(x, 1.0f + __expf(-2.0f * u));
 }
-// GELU-tanh on a float4 with Blackwell's packed fp32 pipe (fma/mul/add .f32x2: two lanes per instruction):
-// y = x / (1 + 2^(c2 * x * (1 + k1 x^2))),  c2 = -2 log2(e) sqrt(2/pi); ex2 / rcp stay scalar MUFU ops.
-__device__ __forceinline__ float4 gelu_tanh_fast4(float4 v) {
+// GELU-tanh on a pair, y = x / (1 + 2^(c2 * x * (1 + k1 x^2))),  c2 = -2 log2(e) sqrt(2/pi), with ex2 / rcp on the MUFU
+// pipe.  Every step is an explicitly rounded single operation (no contraction), so the result does not depend on how the
+// compiler schedules it.
+__device__ __forceinline__ float gelu_tanh_fast1(float x) {
   const float k1 = 0.044715f, c2 = -2.0f * 1.4426950408889634f * 0.7978845608028654f;
-  float4 y;
-  asm("{\n\t"
-      ".reg .b64 xa, xb, ta, tb, ka, ca, one;\n\t"
-      ".reg .f32 e0, e1, e2, e3;\n\t"
-      "mov.b64 xa, {%4, %5};\n\t"
-      "mov.b64 xb, {%6, %7};\n\t"
-      "mov.b64 ka, {%8, %8};\n\t"
-      "mov.b64 ca, {%9, %9};\n\t"
-      "mov.b64 one, {%10, %10};\n\t"
-      "mul.f32x2 ta, xa, xa;\n\t"            // x^2
-      "mul.f32x2 tb, xb, xb;\n\t"
-      "fma.rn.f32x2 ta, ta, ka, one;\n\t"    // 1 + k1 x^2
-      "fma.rn.f32x2 tb, tb, ka, one;\n\t"
-      "mul.f32x2 ta, ta, xa;\n\t"            // x (1 + k1 x^2)
-      "mul.f32x2 tb, tb, xb;\n\t"
-      "mul.f32x2 ta, ta, ca;\n\t"            // exponent (base 2)
-      "mul.f32x2 tb, tb, ca;\n\t"
-      "mov.b64 {e0, e1}, ta;\n\t"
-      "mov.b64 {e2, e3}, tb;\n\t"
-      "ex2.approx.ftz.f32 e0, e0;\n\t"
-      "ex2.approx.ftz.f32 e1, e1;\n\t"
-      "ex2.approx.ftz.f32 e2, e2;\n\t"
-      "ex2.approx.ftz.f32 e3, e3;\n\t"
-      "mov.b64 ta, {e0, e1};\n\t"
-      "mov.b64 tb, {e2, e3};\n\t"
-      "add.f32x2 ta, ta, one;\n\t"           // 1 + e
-      "add.f32x2 tb, tb, one;\n\t"
-      "mov.b64 {e0, e1}, ta;\n\t"
-      "mov.b64 {e2, e3}, tb;\n\t"
-      "rcp.approx.ftz.f32 e0, e0;\n\t"
-      "rcp.approx.ftz.f32 e1, e1;\n\t"
-      "rcp.approx.ftz.f32 e2, e2;\n\t"
-      "rcp.approx.ftz.f32 e3, e3;\n\t"
-      "mov.b64 ta, {e0, e1};\n\t"
-      "mov.b64 tb, {e2, e3};\n\t"
-      "mul.f32x2 ta, ta, xa;\n\t"            // x / (1 + e)
-      "mul.f32x2 tb, tb, xb;\n\t"
-      "mov.b64 {%0, %1}, ta;\n\t"
-      "mov.b64 {%2, %3}, tb;\n\t"
-      "}"
-      : "=f"(y.x), "=f"(y.y), "=f"(y.z), "=f"(y.w)
-      : "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "f"(k1), "f"(c2), "f"(1.0f));
-  return y;
+  float t = __fmul_rn(x, x);                 // x^2
+  t = __fmaf_rn(t, k1, 1.0f);                // 1 + k1 x^2
+  t = __fmul_rn(t, x);                       // x (1 + k1 x^2)
+  t = __fmul_rn(t, c2);                      // exponent (base 2)
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(t));
+  e = __fadd_rn(e, 1.0f);                    // 1 + e
+  asm("rcp.approx.ftz.f32 %0, %0;" : "+f"(e));
+  return __fmul_rn(e, x);                    // x / (1 + e)
 }
+__device__ __forceinline__ float2 gelu_tanh_fast2(float2 v) { return make_float2(gelu_tanh_fast1(v.x), gelu_tanh_fast1(v.y)); }
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + expf(-x)); }
 
 enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_SILU = 2 };
@@ -155,23 +123,20 @@ __device__ __forceinline__ uint32_t pack2_resid_bf16(float a, float b, uint32_t 
   return r;
 }
 
-// packed fp32 pipe (Blackwell FFMA2 / FADD2: one issue slot for two lanes of arithmetic): (d0, d1) = (a0, a1) * (b0, b1) + (c0, c1)
+// element pairs: (d0, d1) = (a0, a1) * (b0, b1) + (c0, c1) and (d0, d1) = (a0, a1) + (b0, b1), each lane rounded once
 __device__ __forceinline__ void ffma2(float a0, float a1, float b0, float b1, float c0, float c1, float& d0, float& d1) {
-  asm("{\n\t.reg .b64 a, b, c;\n\t"
-      "mov.b64 a, {%2, %3};\n\t"
-      "mov.b64 b, {%4, %5};\n\t"
-      "mov.b64 c, {%6, %7};\n\t"
-      "fma.rn.f32x2 a, a, b, c;\n\t"
-      "mov.b64 {%0, %1}, a;\n\t}"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
+  d0 = __fmaf_rn(a0, b0, c0);
+  d1 = __fmaf_rn(a1, b1, c1);
+}
+// the same on pairs held as packed 64-bit registers (low word = first lane): acc = a * b + acc per lane
+__device__ __forceinline__ void fma2_packed(unsigned long long& acc, unsigned long long a, unsigned long long b) {
+  const float d0 = __fmaf_rn(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)acc));
+  const float d1 = __fmaf_rn(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)), __uint_as_float((uint32_t)(acc >> 32)));
+  acc = (unsigned long long)__float_as_uint(d0) | ((unsigned long long)__float_as_uint(d1) << 32);
 }
 __device__ __forceinline__ void fadd2(float a0, float a1, float b0, float b1, float& d0, float& d1) {
-  asm("{\n\t.reg .b64 a, b;\n\t"
-      "mov.b64 a, {%2, %3};\n\t"
-      "mov.b64 b, {%4, %5};\n\t"
-      "add.rn.f32x2 a, a, b;\n\t"
-      "mov.b64 {%0, %1}, a;\n\t}"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fadd_rn(a0, b0);
+  d1 = __fadd_rn(a1, b1);
 }
 
 }  // namespace stk

@@ -3,7 +3,7 @@
 // Host-side orchestration of the encode / decode hot path of mimogpt/infer/SelftokPipeline.py — weights under the
 // reference's checkpoint key names, every input-independent table built once at finalize, one workspace per batch
 // size, and the 50-step sampler captured in one CUDA graph.  All arithmetic is in the kernels of kernels_simt.cu
-// (fp32 FFMA: encoder, VQ, tables), gemm_tc.cu (tcgen05 GEMMs of the MMDiT) and attn_tc5.cu (tcgen05 joint attention).
+// (fp32 FFMA: encoder, VQ, tables), gemm_tc.cu (wgmma GEMMs of the MMDiT) and attn_tc5.cu (wgmma joint attention).
 #include "../../include/selftok_b200.h"
 #include "common.cuh"
 #include "kernels.h"
@@ -177,7 +177,7 @@ static int lin32(selftok_engine* e, const std::string& prefix, const float* A, i
   PROF(PC_LINEAR_F32, launch_linear_f32(A, lda, W->d, K, M, N, K, ep, s));
   return 0;
 }
-// tcgen05 path: A given as bf16 planes
+// tensor-core path: A given as bf16 planes
 static int lintc(selftok_engine* e, const std::string& prefix, const bf16* A_hi, const bf16* A_lo, int64_t M,
                  Epilogue ep, cudaStream_t s) {
   GETW(W, prefix + ".weight");
@@ -193,7 +193,7 @@ static int lintc(selftok_engine* e, const std::string& prefix, const bf16* A_hi,
   return 0;
 }
 
-// tcgen05 problem descriptor for a checkpoint linear (weights already packed at finalize)
+// tensor-core problem descriptor for a checkpoint linear (weights already packed at finalize)
 static int tc_problem(selftok_engine* e, const std::string& prefix, const bf16* A_hi, const bf16* A_lo, int64_t M, Epilogue ep,
                       TcProblem* out) {
   GETW(W, prefix + ".weight");
@@ -216,7 +216,7 @@ static int lintc2(selftok_engine* e, const TcProblem* probs, int n, cudaStream_t
 
 // ------------------------------------------------------------------------------------------------ C ABI: lifetime
 extern "C" __attribute__((visibility("default"))) const char* selftok_last_error(void) { return g_error.c_str(); }
-extern "C" __attribute__((visibility("default"))) const char* selftok_version(void) { return "selftok_b200 abi1 sm_100a (fp32-ffma + tcgen05 kind::f16)"; }
+extern "C" __attribute__((visibility("default"))) const char* selftok_version(void) { return "selftok_b200 abi1 sm_90a (fp32-ffma + wgmma)"; }
 
 extern "C" __attribute__((visibility("default"))) int selftok_create(const selftok_config_t* cfg, selftok_handle_t* out) {
   STK_CHECK(cfg && out, SELFTOK_ERR_BAD_ARG, "selftok_create: null argument");
@@ -229,8 +229,8 @@ extern "C" __attribute__((visibility("default"))) int selftok_create(const selft
   STK_CHECK(cfg->device >= 0 && cfg->device < ndev, SELFTOK_ERR_BAD_ARG, "bad device ordinal");
   cudaDeviceProp prop;
   STK_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) {
-    set_error("device is not sm_100 (Blackwell B200): kernels are built for sm_100a only");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device is not sm_90 (Hopper H100): kernels are built for sm_90a only");
     return SELFTOK_ERR_NO_DEVICE;
   }
   STK_CHECK(cfg->K > 0 && cfg->latent > 0 && cfg->dit_depth > 0 && cfg->enc_depth > 0, SELFTOK_ERR_BAD_ARG, "bad dims");
@@ -977,7 +977,7 @@ static int post_attention(selftok_engine* e, const std::string& blk, float* resi
 }
 
 // x = x_embedder(patches) + cropped pos_embed (mmdit.py:1000-1001) from ws.patch into ws.x.  Tensor-core modes: the K = 64 GEMM on
-// the tcgen05 kernel with split-bf16 operands (fp32-faithful) instead of the fp32 FFMA kernel (0.3 ms -> ~20 us per evaluation).
+// the tensor-core kernel with split-bf16 operands (fp32-faithful) instead of the fp32 FFMA kernel (0.3 ms -> ~20 us per evaluation).
 static int x_embed(selftok_engine* e, int B, cudaStream_t s) {
   const selftok_config_t& c = e->cfg;
   DecodeWs& w = e->dws;

@@ -1,252 +1,111 @@
-// tcgen05 GEMM of the MMDiT linears (sm_100a):  y = A W^T (+bias, fused epilogue), fp32 accumulation in TMEM.
+// Tensor-core GEMM of the MMDiT linears (sm_90a):  y = A W^T (+bias, fused epilogue), fp32 accumulation in registers.
 //
 //   operands   bf16 planes, K-major.  NSPLIT == 1: y = A_hi W_hi^T.  NSPLIT == 3 ("bf16x3", fp32-faithful to ~2^-17):
-//              y = A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T, all three products accumulated into the same TMEM tile.
-//   tile       128 x 256 x 64 per pipeline stage, UMMA 128x256x16 (kind::f16, cta_group::1)
-//   staging    TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) -> shared memory ring, mbarrier full/empty pairs
-//   roles      warp 0: TMA producer (1 thread) | warp 1: MMA issuer (1 thread) | warps 2-9: epilogue (TMEM -> regs -> smem transpose -> HBM)
-//   TMEM       512 columns = 2 accumulator tiles; the epilogue of tile i overlaps the MMAs of tile i+1
-//   schedule   persistent CTAs (grid = #SMs), tiles rasterised in groups of 8 M-blocks for L2 reuse of W
+//              y = A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T, all three products accumulated into the same registers.
+//   tile       128 x 256 x 64 per pipeline stage per CTA; two consumer warpgroups, each wgmma m64n256k16 on its 64 rows
+//   staging    TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared memory ring, mbarrier full/empty pairs
+//   roles      warpgroups 0-1: wgmma + epilogue (registers -> HBM) | warp 8: TMA producer (1 thread)
+//   cluster    CL == 2: two CTAs (rows 256 apart in M) share the W tile: each loads half of it and multicasts it to both,
+//              halving the L2 -> SM traffic of the weights; CL == 1: one CTA loads the whole tile
+//   schedule   persistent CTAs (grid = #SMs), tiles rasterised in groups of M-blocks for L2 reuse of W
 //
 // Replaces the cuBLAS SGEMMs behind nn.Linear in DismantledBlock (sd3/mmdit.py:266,269,293,301; other_impls.py:82-84)
 // together with the elementwise kernels around them (bias, GELU-tanh, gate*y + residual; mmdit.py:485-496).
 #include "common.cuh"
+#include "hopper.cuh"
 #include "kernels.h"
 
-#include <cuda.h>   // CUtensorMap types only; the driver entry point is resolved at run time (no -lcuda)
 #include <stdlib.h>
 
 namespace stk {
 
 namespace {
 
-constexpr int BM = 128, BN = 256, BK = 64, UMMA_K = 16;
+using namespace hop;
+
+constexpr int BM = 128, BN = 256, BK = 64, WK = 16;
 constexpr int A_TILE_BYTES = BM * BK * 2;      // 16 KiB
 constexpr int B_TILE_BYTES = BN * BK * 2;      // 32 KiB
-constexpr int NUM_THREADS = 64 + 8 * 32;     // TMA warp, MMA warp, 8 epilogue warps
-constexpr int TMEM_COLS = 512;
+constexpr int CONSUMERS = 2;                   // warpgroups of 64 rows
+constexpr int NUM_THREADS = CONSUMERS * 128 + 32;
+constexpr int ACC = BN / 2;                    // fp32 accumulators per consumer thread
 
 template <int NSPLIT> struct Cfg {
   static constexpr int PLANES = NSPLIT == 3 ? 2 : 1;
   static constexpr int STAGE_BYTES = PLANES * (A_TILE_BYTES + B_TILE_BYTES);     // 48 KiB / 96 KiB
   static constexpr int STAGES = NSPLIT == 3 ? 2 : 4;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 8 * 32 * 32 * 4 /*epilogue staging*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// ---------------------------------------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// Suspend-time hint: a waiting warp sleeps in hardware until the phase flips (or the hint expires) instead of spinning.
-// Measured on the 96 GEMMs of sampler step 0: 51.0 ms -> 49.1 ms (the eight epilogue warps and the producer no longer burn
-// issue slots and power next to the MMA issuer).
-constexpr uint32_t kSuspendHintNs = 20000;
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(bar), "r"(parity), "r"(kSuspendHintNs) : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug traps (-> CUDA error on the host) instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && clock64() - t0 > 8000000000LL) {
-      printf("selftok gemm_tc: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-      __trap();
-    }
-  }
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major SWIZZLE_128B shared-memory operand descriptor (cute::UMMA::SmemDescriptor layout):
-//   [0,14) start >> 4 | [16,30) LBO >> 4 (=1, unused for swizzled K-major) | [32,46) SBO >> 4 (8 rows * 128 B = 1024)
-//   [46,48) version = 1 (sm_100) | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D fp32 (bits 4-5 = 1), A/B bf16 (bits 7-9, 10-12 = 1),
-// both K-major (bits 15, 16 = 0), N >> 3 at bit 17, M >> 4 at bit 24.
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n, int fp16) {
-  const uint32_t fmt = fp16 ? 0u : 1u;                   // F16F32Format: F16 = 0, BF16 = 1
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ void wgmma_tile(float (&d)[ACC], uint64_t da, uint64_t db, uint32_t acc, bool fp16) {
+  if (fp16) wgmma_m64n256k16_ss_f16(d, da, db, acc);
+  else wgmma_m64n256k16_ss_bf16(d, da, db, acc);
 }
 
-// Epilogue of one 32-row x 128-column accumulator block (TMEM lane quarter x column half), executed by one warp;
-// 8 epilogue warps cover the 128 x 256 tile.  tcgen05.ld hands lane i row i of a 32 x 32 chunk; the chunk is transposed
-// through an XOR-swizzled shared-memory tile (conflict-free 128-bit writes and reads) so that every global access of
-// the warp covers four full 128-byte row segments (8 lanes x float4 per row).  For the gated-residual epilogue all
-// residual / gate loads of a chunk are issued BEFORE the TMEM read: one memory latency per chunk, not one per row.
-// (A lane-per-row epilogue touches 32 cache lines per instruction with nothing in flight and made the LSU, not the
-// tensor pipe, the limiter of the first version of this kernel.)
-constexpr int EPI_STAGE_FLOATS = 32 * 32;
-constexpr int EPI_WARPS = 8;
-__device__ __forceinline__ float4 ldg4(const float* p) { return *reinterpret_cast<const float4*>(p); }
-// two fp32 -> packed 16-bit pair (IEEE half, saturating, or bf16): one cvt per pair
-__device__ __forceinline__ uint32_t pack2(float lo, float hi, bool fp16) { return pack2_sat16(lo, hi, fp16); }
-// MODE / GELU are compile-time so that the per-element path carries no mode branches; the arithmetic of all 8 row passes
-// of a chunk is issued unconditionally (independent chains -> ILP) and only the global stores are predicated.
+__device__ __forceinline__ float2 ldg2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+
+// Epilogue of one consumer thread's accumulators: rows row0 and row0 + 8, column pairs col0 + 8 j (j < 32).  Every access of
+// a quad of lanes covers 32 contiguous bytes of a row.  MODE / GELU are compile-time so that the per-element path carries no
+// mode branches.
 template <int MODE, bool GELU>
-__device__ __forceinline__ void epilogue_block(const Epilogue& e, uint32_t tmem_addr, float* stage, int lane,
-                                               int64_t m_base, int64_t M, int n_first, int N) {
-  const int rsub = lane >> 3, cq = lane & 7;            // pass k: row 4k + rsub of the chunk; this lane's 4 columns
+__device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&acc)[ACC], int64_t row0, int64_t M, int col0, int N) {
   const bool per_row_gate = MODE == EPI_RESID && e.gate && e.gate_period > 1;
   const bool per_row_add = MODE == EPI_STORE && e.addtab;
   const bool fp16 = e.fp16 != 0;
-  int orow_[8];                                          // output row (32-bit; the 64-bit offset is formed at the access)
-  int mrow[8];
-  bool rvalid[8];
+  int orow[2], mrow[2];
+  bool rvalid[2];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int64_t m = m_base + 4 * k + rsub;
-    rvalid[k] = m < M;
+  for (int r = 0; r < 2; ++r) {
+    const int64_t m = row0 + 8 * r;
+    rvalid[r] = m < M;
     const int mi = (int)m;
-    const int orow = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
-    orow_[k] = orow;
-    mrow[k] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
+    orow[r] = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
+    mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
   }
-#pragma unroll 1
-  for (int c = 0; c < (BN / 2) / 32; ++c) {
-    const int n0 = n_first + c * 32;
-    if (n0 >= N) break;                                 // warp-uniform
-    const int n = n0 + cq * 4;
-    const bool col_ok = n < N;                          // N % 4 == 0: a float4 group is all in or all out
-    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 bias = (e.bias && col_ok) ? ldg4(e.bias + n) : zero4;
-    float4 res[8], gt[8];
-    if (MODE == EPI_RESID) {
-      const float4 g0 = (e.gate && !per_row_gate && col_ok) ? ldg4(e.gate + n) : make_float4(1.f, 1.f, 1.f, 1.f);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const bool ok = col_ok && rvalid[k];
-        res[k] = ok ? ldg4(e.resid + (int64_t)orow_[k] * e.ldo + n) : zero4;
-        gt[k] = (per_row_gate && ok) ? ldg4(e.gate + (int64_t)mrow[k] * e.gate_ld + n) : g0;
-      }
-    }
-    uint32_t r[32];
-    tmem_ld32(tmem_addr + (uint32_t)(c * 32), r);
-    tmem_ld_wait();
-    __syncwarp();                                       // previous chunk fully read back
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = col0 + 8 * j;
+    if (n >= N) continue;                               // N % 4 == 0 and n even: a pair is all in or all out
+    const float2 bias = e.bias ? ldg2(e.bias + n) : make_float2(0.f, 0.f);
+    const float2 g0 = (MODE == EPI_RESID && e.gate && !per_row_gate) ? ldg2(e.gate + n) : make_float2(1.f, 1.f);
 #pragma unroll
-    for (int q = 0; q < 8; ++q)
-      *reinterpret_cast<uint4*>(&stage[lane * 32 + ((q ^ (lane & 7)) << 2)]) = make_uint4(r[4 * q], r[4 * q + 1], r[4 * q + 2], r[4 * q + 3]);
-    __syncwarp();
-    float4 y[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int row = 4 * k + rsub;
-      // (a timing-only build that skipped this shared-memory transpose was 4.6 % faster: the staging is not the bottleneck)
-      const float4 v = *reinterpret_cast<const float4*>(&stage[row * 32 + ((cq ^ (row & 7)) << 2)]);
-      y[k] = make_float4(v.x + bias.x, v.y + bias.y, v.z + bias.z, v.w + bias.w);
-      if (GELU) y[k] = gelu_tanh_fast4(y[k]);
+    for (int r = 0; r < 2; ++r) {
+      if (!rvalid[r]) continue;
+      float2 y = make_float2(acc[4 * j + 2 * r] + bias.x, acc[4 * j + 2 * r + 1] + bias.y);
+      if (GELU) y = gelu_tanh_fast2(y);
+      const int64_t o = (int64_t)orow[r] * e.ldo + n;
       if (MODE == EPI_RESID) {
-        y[k].x = fmaf(gt[k].x, y[k].x, res[k].x); y[k].y = fmaf(gt[k].y, y[k].y, res[k].y);
-        y[k].z = fmaf(gt[k].z, y[k].z, res[k].z); y[k].w = fmaf(gt[k].w, y[k].w, res[k].w);
+        const float2 res = ldg2(e.resid + o);
+        const float2 gt = per_row_gate ? ldg2(e.gate + (int64_t)mrow[r] * e.gate_ld + n) : g0;
+        y.x = fmaf(gt.x, y.x, res.x); y.y = fmaf(gt.y, y.y, res.y);
       }
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (!(col_ok && rvalid[k])) continue;
-      const int64_t o = (int64_t)orow_[k] * e.ldo + n;
       if (MODE == EPI_SPLIT) {
-        *reinterpret_cast<uint2*>(e.out_hi + o) = make_uint2(pack2(y[k].x, y[k].y, fp16), pack2(y[k].z, y[k].w, fp16));
+        const uint32_t hi = pack2_sat16(y.x, y.y, fp16);
+        *reinterpret_cast<uint32_t*>(e.out_hi + o) = hi;
         if (e.out_lo) {                                  // bf16x3: residual planes
-          const float lx = y[k].x - __bfloat162float(__float2bfloat16_rn(y[k].x)), ly = y[k].y - __bfloat162float(__float2bfloat16_rn(y[k].y));
-          const float lz = y[k].z - __bfloat162float(__float2bfloat16_rn(y[k].z)), lw = y[k].w - __bfloat162float(__float2bfloat16_rn(y[k].w));
-          *reinterpret_cast<uint2*>(e.out_lo + o) = make_uint2(pack2(lx, ly, false), pack2(lz, lw, false));
+          const float lx = y.x - __bfloat162float(__float2bfloat16_rn(y.x)), ly = y.y - __bfloat162float(__float2bfloat16_rn(y.y));
+          *reinterpret_cast<uint32_t*>(e.out_lo + o) = pack2_sat16(lx, ly, false);
         }
       } else {
         if (per_row_add) {
-          const float4 a = ldg4(e.addtab + (int64_t)mrow[k] * e.add_ld + n);
-          y[k].x += a.x; y[k].y += a.y; y[k].z += a.z; y[k].w += a.w;
+          const float2 a = ldg2(e.addtab + (int64_t)mrow[r] * e.add_ld + n);
+          y.x += a.x; y.y += a.y;
         }
-        *reinterpret_cast<float4*>(e.out + o) = y[k];
+        *reinterpret_cast<float2*>(e.out + o) = y;
       }
     }
-  }
-}
-
-// Issued by the epilogue warps BEFORE they wait for the accumulator: pulls this warp's 32 x 128 residual block (and its
-// per-row gate rows) into L2 while the MMAs of the tile are still running, so the gated-residual loads of the epilogue hit L2
-// instead of paying the HBM latency once per chunk (long-scoreboard stalls were 37 % of the epilogue's samples).
-__device__ __forceinline__ void epilogue_prefetch(const Epilogue& e, int lane, int64_t m_base, int64_t M, int n_first, int N) {
-  if (e.mode != EPI_RESID) return;
-  const int64_t m = m_base + lane;
-  if (m >= M || n_first >= N) return;
-  const int mi = (int)m;
-  const int orow = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
-  const float* rp = e.resid + (int64_t)orow * e.ldo + n_first;
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    if (n_first + j * 32 < N) asm volatile("prefetch.global.L2 [%0];" ::"l"(rp + j * 32));
-  if (e.gate && e.gate_period > 1) {
-    const float* gp = e.gate + (int64_t)(mi % e.gate_period) * e.gate_ld + n_first;
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (n_first + j * 32 < N) asm volatile("prefetch.global.L2 [%0];" ::"l"(gp + j * 32));
   }
 }
 
 // mode / activation dispatch (uniform across the grid)
-__device__ __forceinline__ void epilogue_dispatch(const Epilogue& e, uint32_t tmem_addr, float* stage, int lane, int64_t m_base,
-                                                  int64_t M, int n_first, int N) {
-  if (e.mode == EPI_RESID) epilogue_block<EPI_RESID, false>(e, tmem_addr, stage, lane, m_base, M, n_first, N);
+__device__ __forceinline__ void epilogue_dispatch(const Epilogue& e, const float (&acc)[ACC], int64_t row0, int64_t M, int col0, int N) {
+  if (e.mode == EPI_RESID) epilogue_tile<EPI_RESID, false>(e, acc, row0, M, col0, N);
   else if (e.mode == EPI_SPLIT) {
-    if (e.act == ACT_GELU) epilogue_block<EPI_SPLIT, true>(e, tmem_addr, stage, lane, m_base, M, n_first, N);
-    else epilogue_block<EPI_SPLIT, false>(e, tmem_addr, stage, lane, m_base, M, n_first, N);
+    if (e.act == ACT_GELU) epilogue_tile<EPI_SPLIT, true>(e, acc, row0, M, col0, N);
+    else epilogue_tile<EPI_SPLIT, false>(e, acc, row0, M, col0, N);
   } else {
-    if (e.act == ACT_GELU) epilogue_block<EPI_STORE, true>(e, tmem_addr, stage, lane, m_base, M, n_first, N);
-    else epilogue_block<EPI_STORE, false>(e, tmem_addr, stage, lane, m_base, M, n_first, N);
+    if (e.act == ACT_GELU) epilogue_tile<EPI_STORE, true>(e, acc, row0, M, col0, N);
+    else epilogue_tile<EPI_STORE, false>(e, acc, row0, M, col0, N);
   }
 }
 
@@ -268,223 +127,12 @@ struct GemmParams {
   // tap (dy, dx) reads phase (dy & 1, dx & 1) shifted by (dy >> 1, dx >> 1) -- unit-stride boxes again, the zero fill past the last
   // row / column is the one-sided padding.  conv_H / conv_W are the OUTPUT dims.
   int conv_C = 0, conv_H = 0, conv_W = 0, conv_stride = 1;
-  int raster_gm = 4;     // pair-rows per raster group of the SM-pair kernel (pair_coords)
+  int raster_gm = 4;     // cluster-rows per raster group (tile_coords)
 };
 
-__device__ __forceinline__ void tile_coords(int t, int m_tiles, int n_tiles, int& m_blk, int& n_blk) {
-  constexpr int GM = 8;
-  const int per_group = GM * n_tiles;
-  const int group = t / per_group;
-  const int first_m = group * GM;
-  const int gm = min(GM, m_tiles - first_m);
-  const int local = t - group * per_group;
-  m_blk = first_m + local % gm;
-  n_blk = local / gm;
-}
-
-// ---------------------------------------------------------------------------------------------- kernel
-template <int NSPLIT>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-               const GemmParams p) {
-  using C = Cfg<NSPLIT>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;           // SWIZZLE_128B tiles need 1024 B alignment
-  const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (int)((p.M + BM - 1) / BM), n_tiles = (p.N + BN - 1) / BN;
-  const int num_tiles = m_tiles * n_tiles;
-  const int nk = (p.K + BK - 1) / BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_a_hi);
-    tma_prefetch_desc(&map_b_hi);
-    if (NSPLIT == 3) { tma_prefetch_desc(&map_a_lo); tma_prefetch_desc(&map_b_lo); }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), EPI_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"((uint32_t)TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp == 0) {
-    // =========================================================== TMA producer
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int m_blk, n_blk;
-        tile_coords(t, m_tiles, n_tiles, m_blk, n_blk);
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t fb = full_bar(stage);
-          mbar_expect_tx(fb, C::STAGE_BYTES);
-          tma_load_2d(sa, &map_a_hi, fb, kb * BK, m_blk * BM);
-          tma_load_2d(sa + C::PLANES * A_TILE_BYTES, &map_b_hi, fb, kb * BK, n_blk * BN);
-          if (NSPLIT == 3) {
-            tma_load_2d(sa + A_TILE_BYTES, &map_a_lo, fb, kb * BK, m_blk * BM);
-            tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_b_lo, fb, kb * BK, n_blk * BN);
-          }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // =========================================================== MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BM, BN, p.fp16);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1);               // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * BN;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa_hi = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t sb_hi = sa_hi + C::PLANES * A_TILE_BYTES;
-          const uint32_t sa_lo = sa_hi + A_TILE_BYTES;
-          const uint32_t sb_lo = sb_hi + B_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint32_t koff = k * UMMA_K * 2;                // bytes inside the 128 B swizzle row
-            const uint64_t da_hi = make_smem_desc(sa_hi + koff), db_hi = make_smem_desc(sb_hi + koff);
-            tc_mma_f16(d_tmem, da_hi, db_hi, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            if (NSPLIT == 3) {
-              const uint64_t da_lo = make_smem_desc(sa_lo + koff), db_lo = make_smem_desc(sb_lo + koff);
-              tc_mma_f16(d_tmem, da_hi, db_lo, idesc, 1u);
-              tc_mma_f16(d_tmem, da_lo, db_hi, idesc, 1u);
-            }
-          }
-          tc_commit(empty_bar(stage));                           // smem slot reusable once these MMAs retire
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit(tfull_bar(acc));                               // accumulator complete -> epilogue
-      }
-    }
-  } else {
-    // =========================================================== epilogue warps 2..9 (TMEM lane quarter = warp % 4, column half = (warp-2)/4)
-    const int quarter = warp & 3, half = (warp - 2) >> 2;        // TMEM lane quarter = warp % 4; column half
-    const Epilogue& e = p.ep;
-    float* stage = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - smem_u32(smem_raw))) + (warp - 2) * EPI_STAGE_FLOATS;
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      int m_blk, n_blk;
-      tile_coords(t, m_tiles, n_tiles, m_blk, n_blk);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      epilogue_prefetch(e, lane, (int64_t)m_blk * BM + quarter * 32, p.M, n_blk * BN + half * (BN / 2), p.N);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      epilogue_dispatch(e, tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + half * (BN / 2)), stage, lane,
-                     (int64_t)m_blk * BM + quarter * 32, p.M, n_blk * BN + half * (BN / 2), p.N);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-    }
-  }
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------- 2-CTA kernel
-// cta_group::2: a cluster of two CTAs (one SM pair) computes a 256 x 256 output tile with UMMA 256x256x16.  Each CTA
-// stages its own 128 A rows and HALF of the W tile (128 of the 256 N rows); the tensor cores of the pair exchange the
-// halves, so per SM the shared-memory traffic (TMA fill + operand reads) drops from 156-192 B/clk to 104-128 B/clk and the
-// L2 -> SM bytes per FLOP halve.  Only the leader CTA (cluster rank 0) issues MMAs.
-//   full[s]    lives in the leader; both CTAs' TMA loads complete_tx on it (peer bit of the barrier address cleared)
-//   empty[s]   one per CTA; the leader's tcgen05.commit multicasts the arrive to both
-//   tfull[a]   one per CTA (multicast commit); tempty[a] lives in the leader and counts the 8 epilogue warps of the pair
-template <int NSPLIT> struct Cfg2 {
-  static constexpr int PLANES = NSPLIT == 3 ? 2 : 1;
-  static constexpr int HALF_B_BYTES = (BN / 2) * BK * 2;                                 // 16 KiB
-  static constexpr int STAGE_BYTES = PLANES * (A_TILE_BYTES + HALF_B_BYTES);             // 32 KiB / 64 KiB per CTA
-  static constexpr int STAGES = NSPLIT == 3 ? 3 : 6;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + 8 * 32 * 32 * 4;
-};
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-// The weight tile is re-read by every group of M tiles; without a hint the activation / residual / output streams of the
-// K = 6144 GEMM push it out of L2 between groups (fc2: 1.69 GB of DRAM reads for 0.93 GB algorithmic).  evict_last keeps it.
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm_hint(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1,
-                                                     uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc2(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on the barrier at the same offset in CTA `rank` of the cluster.  Default semantics (.release at CTA scope), as
-// CUTLASS's ClusterBarrier::arrive: the barrier only hands the TMEM accumulator back to the MMA issuer, and the TMEM reads
-// are already complete (tcgen05.wait::ld) and ordered (tcgen05.fence::before_thread_sync).  The explicit .release.cluster
-// form used in round 1 compiled to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR in front of the arrive -- it drained the warp's
-// outstanding global stores first and held 6-9 % of all warp samples in every GEMM (profiles/r1_layer_ncu_full_final.md).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t local_bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(local_bar), "r"(rank) : "memory");
-}
-
-__device__ __forceinline__ void pair_coords(int t, int pm_tiles, int n_tiles, int GM, int& pm, int& n_blk) {
-  // GM pair-rows (default 4 = 1024 A rows) share each W tile in L2; SELFTOK_GEMM_GM is a measurement knob (any value is a
-  // bijection of the tile list, results never change)
+__device__ __forceinline__ void tile_coords(int t, int pm_tiles, int n_tiles, int GM, int& pm, int& n_blk) {
+  // GM cluster-rows share each W tile in L2; SELFTOK_GEMM_GM is a measurement knob (any value is a bijection of the tile
+  // list, results never change)
   const int per_group = GM * n_tiles;
   const int group = t / per_group;
   const int first = group * GM;
@@ -494,33 +142,33 @@ __device__ __forceinline__ void pair_coords(int t, int pm_tiles, int n_tiles, in
   n_blk = local / gm;
 }
 
-template <int NSPLIT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_tc2_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcMaps maps1, const GemmParams p0,
-                const GemmParams p1) {
-  // Up to two independent problems (same NSPLIT / operand type) share the launch: the context- and the image-stream GEMM of
-  // a layer.  Tiles of problem 0 come first; problem 1 may be empty (M == 0).
-  using C = Cfg2<NSPLIT>;
+// ---------------------------------------------------------------------------------------------- kernel
+// Up to two independent problems (same NSPLIT / operand type) share the launch: the context- and the image-stream GEMM of
+// a layer.  Tiles of problem 0 come first; problem 1 may be empty (M == 0).  A tile is CL x 128 rows x 256 columns: CTA
+// `rank` of the cluster computes rows [128 rank, 128 rank + 128) of it.
+//   full[s]    per CTA: its own A box plus both halves of the W tile (one from each CTA of the cluster) complete_tx on it
+//   empty[s]   per CTA: counts the two consumer warpgroups of EVERY CTA of the cluster, because the producer of this CTA
+//              writes its half of the W tile into all of them
+template <int NSPLIT, int CL, bool FP16>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcMaps maps1, const GemmParams p0, const GemmParams p1) {
+  static_assert(NSPLIT == 1 || !FP16, "the fp16 mode is single-pass");
+  using C = Cfg<NSPLIT>;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;           // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pm_tiles0 = (int)((p0.M + 2 * BM - 1) / (2 * BM)), n_tiles0 = (p0.N + BN - 1) / BN;
-  const int pm_tiles1 = (int)((p1.M + 2 * BM - 1) / (2 * BM)), n_tiles1 = (p1.N + BN - 1) / BN;
+  const uint32_t rank = CL > 1 ? cluster_ctarank() : 0;
+  const int pm_tiles0 = (int)((p0.M + CL * BM - 1) / (CL * BM)), n_tiles0 = (p0.N + BN - 1) / BN;
+  const int pm_tiles1 = (int)((p1.M + CL * BM - 1) / (CL * BM)), n_tiles1 = (p1.N + BN - 1) / BN;
   const int tiles0 = pm_tiles0 * n_tiles0;
   const int num_tiles = tiles0 + pm_tiles1 * n_tiles1;
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
+  const int cluster_id = blockIdx.x / CL, num_clusters = gridDim.x / CL;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == CONSUMERS * 4 && lane == 0) {
     tma_prefetch_desc(&maps0.a_hi);
     tma_prefetch_desc(&maps0.b_hi);
     if (NSPLIT == 3) { tma_prefetch_desc(&maps0.a_lo); tma_prefetch_desc(&maps0.b_lo); }
@@ -529,37 +177,29 @@ gemm_tc2_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ Tc
       tma_prefetch_desc(&maps1.b_hi);
       if (NSPLIT == 3) { tma_prefetch_desc(&maps1.a_lo); tma_prefetch_desc(&maps1.b_lo); }
     }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 2 * EPI_WARPS); }
+    for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMERS * CL); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"((uint32_t)TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();                                     // peer barriers initialised before any remote arrive / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  if (CL > 1) cluster_sync_all();                         // peer barriers initialised before any multicast / remote arrive
 
-  if (warp == 0) {
-    // =========================================================== TMA producer (both CTAs)
-    if (lane == 0) {
+  if (warp >= CONSUMERS * 4) {
+    // =========================================================== TMA producer
+    if (warp == CONSUMERS * 4 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
+      // The weight tile is re-read by every group of M tiles; without a hint the activation / residual / output streams of the
+      // K = 6144 GEMM push it out of L2 between groups.  evict_last keeps it.
       const uint64_t w_policy = l2_policy_evict_last();
       for (int t = cluster_id; t < num_tiles; t += num_clusters) {
         const bool second = t >= tiles0;
         const TcMaps& mp = second ? maps1 : maps0;
-        int pm, n_blk;
-        if (second) pair_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
-        else pair_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
         const GemmParams& pp = second ? p1 : p0;
+        int pm, n_blk;
+        if (second) tile_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
+        else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
         const int nk = (pp.K + BK - 1) / BK;
-        const int m_row = pm * 2 * BM + (int)rank * BM;            // this CTA's 128 A rows
-        const int n_row = n_blk * BN + (int)rank * (BN / 2);       // this CTA's half of the W tile
+        const int m_row = (pm * CL + (int)rank) * BM;               // this CTA's 128 A rows
+        const int n_row = n_blk * BN + (int)rank * (BN / CL);       // this CTA's share of the W tile
         // convolution: the 128 rows are 128 / bw image rows of bw pixels starting at (cb, cy, cx)
         const int chunks = pp.conv_C > 0 ? pp.conv_C / BK : 1;
         int cx = 0, cy = 0, cb = 0;
@@ -571,103 +211,88 @@ gemm_tc2_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ Tc
         for (int kb = 0; kb < nk; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1);
           const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t fb = full_bar(stage) & 0xFEFFFFFFu;       // leader's barrier (peer bit cleared)
-          if (leader) mbar_expect_tx(full_bar(stage), 2 * C::STAGE_BYTES);
+          const uint32_t sb = sa + C::PLANES * A_TILE_BYTES + (uint32_t)rank * (B_TILE_BYTES / CL);
+          const uint32_t fb = full_bar(stage);
+          mbar_expect_tx(fb, C::STAGE_BYTES);
           if (pp.conv_C > 0) {
             const int tap = kb / chunks, c0 = (kb - tap * chunks) * BK;
             const int dy = tap / 3, dx = tap - dy * 3;
             int x0 = cx + dx - 1, y0 = cy + dy - 1, n0 = cb;
             if (pp.conv_stride == 2) { x0 = cx + (dx >> 1); y0 = cy + (dy >> 1); n0 = cb * 4 + (dy & 1) * 2 + (dx & 1); }
-            tma_load_4d_2sm(sa, &mp.a_hi, fb, c0, x0, y0, n0);
-            if (NSPLIT == 3) tma_load_4d_2sm(sa + A_TILE_BYTES, &mp.a_lo, fb, c0, x0, y0, n0);
+            tma_load_4d(sa, &mp.a_hi, fb, c0, x0, y0, n0);
+            if (NSPLIT == 3) tma_load_4d(sa + A_TILE_BYTES, &mp.a_lo, fb, c0, x0, y0, n0);
           } else {
-            tma_load_2d_2sm(sa, &mp.a_hi, fb, kb * BK, m_row);
-            if (NSPLIT == 3) tma_load_2d_2sm(sa + A_TILE_BYTES, &mp.a_lo, fb, kb * BK, m_row);
+            tma_load_2d(sa, &mp.a_hi, fb, kb * BK, m_row);
+            if (NSPLIT == 3) tma_load_2d(sa + A_TILE_BYTES, &mp.a_lo, fb, kb * BK, m_row);
           }
-          tma_load_2d_2sm_hint(sa + C::PLANES * A_TILE_BYTES, &mp.b_hi, fb, kb * BK, n_row, w_policy);
-          if (NSPLIT == 3) tma_load_2d_2sm_hint(sa + 2 * A_TILE_BYTES + C::HALF_B_BYTES, &mp.b_lo, fb, kb * BK, n_row, w_policy);
+          if (CL > 1) {
+            tma_load_2d_mc(sb, &mp.b_hi, fb, kb * BK, n_row, (uint16_t)((1u << CL) - 1), w_policy);
+            if (NSPLIT == 3) tma_load_2d_mc(sb + B_TILE_BYTES, &mp.b_lo, fb, kb * BK, n_row, (uint16_t)((1u << CL) - 1), w_policy);
+          } else {
+            tma_load_2d_hint(sb, &mp.b_hi, fb, kb * BK, n_row, w_policy);
+            if (NSPLIT == 3) tma_load_2d_hint(sb + B_TILE_BYTES, &mp.b_lo, fb, kb * BK, n_row, w_policy);
+          }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // =========================================================== MMA issuer (leader CTA only)
-    if (leader && lane == 0) {
-      const uint32_t idesc = make_idesc(2 * BM, BN, p0.fp16);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int t = cluster_id; t < num_tiles; t += num_clusters, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        const int nk = ((t >= tiles0 ? p1.K : p0.K) + BK - 1) / BK;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * BN;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa_hi = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t sb_hi = sa_hi + C::PLANES * A_TILE_BYTES;
-          const uint32_t sa_lo = sa_hi + A_TILE_BYTES;
-          const uint32_t sb_lo = sb_hi + C::HALF_B_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint32_t koff = k * UMMA_K * 2;
-            const uint64_t da_hi = make_smem_desc(sa_hi + koff), db_hi = make_smem_desc(sb_hi + koff);
-            tc_mma_f16_2sm(d_tmem, da_hi, db_hi, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            if (NSPLIT == 3) {
-              const uint64_t da_lo = make_smem_desc(sa_lo + koff), db_lo = make_smem_desc(sb_lo + koff);
-              tc_mma_f16_2sm(d_tmem, da_hi, db_lo, idesc, 1u);
-              tc_mma_f16_2sm(d_tmem, da_lo, db_hi, idesc, 1u);
-            }
-          }
-          tc_commit_mc2(empty_bar(stage));                         // frees the slot in BOTH CTAs
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_mc2(tfull_bar(acc));                             // accumulator ready in BOTH CTAs
       }
     }
   } else {
-    // =========================================================== epilogue warps 2..9 of both CTAs
-    const int quarter = warp & 3, half = (warp - 2) >> 2;        // TMEM lane quarter = warp % 4; column half
-    float* stage = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - smem_u32(smem_raw))) + (warp - 2) * EPI_STAGE_FLOATS;
-    int it = 0;
-    for (int t = cluster_id; t < num_tiles; t += num_clusters, ++it) {
+    // =========================================================== consumer warpgroups: wgmma + epilogue
+    const int wg = warp >> 2;                                        // rows [64 wg, 64 wg + 64) of the CTA's 128
+    const bool signaller = (threadIdx.x & 127) == 0;
+    auto release = [&](int s) {                                      // the stage's wgmma reads have completed
+      if (!signaller) return;
+      if (CL == 1) mbar_arrive(empty_bar(s));
+      else for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_bar(s), (uint32_t)r);
+    };
+    int stage = 0; uint32_t phase = 0;
+    for (int t = cluster_id; t < num_tiles; t += num_clusters) {
       const bool second = t >= tiles0;
       int pm, n_blk;
-      if (second) pair_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
-      else pair_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int64_t m_base = (int64_t)pm * 2 * BM + (int64_t)rank * BM + quarter * 32;
-      const int n_first = n_blk * BN + half * (BN / 2);
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + half * (BN / 2));
-      // the two problems are handled by separate (statically addressed) copies of the epilogue: selecting the parameter block
-      // dynamically costs registers in the hottest loop of the kernel
-      if (!second) {
-        epilogue_prefetch(p0.ep, lane, m_base, p0.M, n_first, p0.N);
-        mbar_wait(tfull_bar(acc), acc_phase);
-        tc_fence_after();
-        epilogue_dispatch(p0.ep, taddr, stage, lane, m_base, p0.M, n_first, p0.N);
-      } else {
-        epilogue_prefetch(p1.ep, lane, m_base, p1.M, n_first, p1.N);
-        mbar_wait(tfull_bar(acc), acc_phase);
-        tc_fence_after();
-        epilogue_dispatch(p1.ep, taddr, stage, lane, m_base, p1.M, n_first, p1.N);
+      if (second) tile_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
+      else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
+      const int nk = ((second ? p1.K : p0.K) + BK - 1) / BK;
+      float acc[ACC];
+#pragma unroll
+      for (int i = 0; i < ACC; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < nk; ++kb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t sa_hi = smem_base + stage * C::STAGE_BYTES + wg * (64 * 128);
+        const uint32_t sa_lo = sa_hi + A_TILE_BYTES;
+        const uint32_t sb_hi = smem_base + stage * C::STAGE_BYTES + C::PLANES * A_TILE_BYTES;
+        const uint32_t sb_lo = sb_hi + B_TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WK; ++k) {
+          const uint32_t koff = k * WK * 2;                          // bytes inside the 128 B swizzle row
+          const uint64_t da_hi = make_smem_desc(sa_hi + koff), db_hi = make_smem_desc(sb_hi + koff);
+          wgmma_tile(acc, da_hi, db_hi, (kb > 0 || k > 0) ? 1u : 0u, FP16);
+          if (NSPLIT == 3) {
+            const uint64_t da_lo = make_smem_desc(sa_lo + koff), db_lo = make_smem_desc(sb_lo + koff);
+            wgmma_tile(acc, da_hi, db_lo, 1u, false);
+            wgmma_tile(acc, da_lo, db_hi, 1u, false);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                             // the previous stage's MMAs have retired
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(tempty_bar(acc), 0);       // the leader's barrier counts all 8 epilogue warps
+      wgmma_wait<0>();
+      fence_regs(acc);
+      release(prev);
+      const int wl = threadIdx.x & 127;
+      const int64_t row0 = (int64_t)(pm * CL + (int)rank) * BM + wg * 64 + (wl >> 5) * 16 + ((wl & 31) >> 2);
+      const int col0 = n_blk * BN + 2 * (wl & 3);
+      // the two problems are handled by separate (statically addressed) copies of the epilogue
+      if (!second) epilogue_dispatch(p0.ep, acc, row0, p0.M, col0, p0.N);
+      else epilogue_dispatch(p1.ep, acc, row0, p1.M, col0, p1.N);
     }
   }
-  // ---- teardown: nobody may exit (or free TMEM) while the peer can still touch its barriers / shared memory
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS) : "memory");
-  }
+  // ---- teardown: nobody may exit while a peer can still multicast into its shared memory or arrive on its barriers
+  if (CL > 1) cluster_sync_all();
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -680,7 +305,7 @@ constexpr int kMaxDev = 64;
 int g_num_sms_dev[kMaxDev];
 bool g_attr_dev[kMaxDev];
 int g_raster_gm = 4;      // SELFTOK_GEMM_GM (measurement knob)
-int g_gemm_ctas = 2;      // 2: cta_group::2 pair kernel (default); 1: single-CTA kernel (SELFTOK_GEMM_CTAS=1)
+int g_gemm_ctas = 2;      // 2: two-CTA clusters sharing the W tile (default); 1: one CTA per tile (SELFTOK_GEMM_CTAS=1)
 
 int make_map(CUtensorMap* map, const __nv_bfloat16* ptr, int64_t rows, int K, int box_rows, int fp16) {
   cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
@@ -758,10 +383,12 @@ int gemm_tc_init() {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   STK_CUDA(cudaDeviceGetAttribute(&g_num_sms_dev[dev], cudaDevAttrMultiProcessorCount, dev));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg2<1>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc2_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg2<3>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
   g_attr_dev[dev] = true;
   return 0;
 }
@@ -804,6 +431,31 @@ static int make_maps(TcMaps* m, const TcProblem& q, int nsplit, int fp16, int b_
   return 0;
 }
 
+template <int NSPLIT, int CL, bool FP16>
+static int launch_kernel(const TcMaps& m0, const TcMaps& m1, const GemmParams& p0, const GemmParams& p1, int clusters, cudaStream_t s) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(CL * clusters);
+  cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = Cfg<NSPLIT>::SMEM_BYTES;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  STK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<NSPLIT, CL, FP16>, m0, m1, p0, p1));
+  count_launch();
+  return 0;
+}
+
+template <int CL>
+static int launch_cl(const TcMaps& m0, const TcMaps& m1, const GemmParams& p0, const GemmParams& p1, int clusters, int nsplit, int fp16,
+                     cudaStream_t s) {
+  if (nsplit == 3) return launch_kernel<3, CL, false>(m0, m1, p0, p1, clusters, s);
+  if (fp16) return launch_kernel<1, CL, true>(m0, m1, p0, p1, clusters, s);
+  return launch_kernel<1, CL, false>(m0, m1, p0, p1, clusters, s);
+}
+
 // One launch for up to two independent problems (the context- and the image-stream GEMM of an MMDiT layer): their tiles share
 // the persistent grid, so the small N = 1536 GEMMs no longer pay a partially filled last wave each.
 int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream_t s, int fp16) {
@@ -813,25 +465,9 @@ int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream
   STK_CUDA(cudaGetDevice(&dev));
   const int g_num_sms = g_num_sms_dev[dev];
   for (int i = 0; i < n; ++i) STK_TRY(check_problem(probs[i], nsplit, fp16));
-  const bool pair = g_gemm_ctas == 2 && g_num_sms >= 2;
-  for (int i = 0; i < n; ++i) STK_CHECK(pair || probs[i].conv_C == 0, -2, "gemm_tc conv: only the SM-pair kernel stages NHWC tiles");
-  if (!pair) {                                            // single-CTA bisecting kernel: one launch per problem
-    for (int i = 0; i < n; ++i) {
-      const TcProblem& q = probs[i];
-      TcMaps m;
-      STK_TRY(make_maps(&m, q, nsplit, fp16, BN));
-      GemmParams p{q.M, q.N, q.K, fp16, q.ep};
-      const int tiles = (int)((q.M + BM - 1) / BM) * ((q.N + BN - 1) / BN);
-      const int grid = tiles < g_num_sms ? tiles : g_num_sms;
-      if (nsplit == 3) gemm_tc_kernel<3><<<grid, NUM_THREADS, Cfg<3>::SMEM_BYTES, s>>>(m.a_hi, m.a_lo, m.b_hi, m.b_lo, p);
-      else gemm_tc_kernel<1><<<grid, NUM_THREADS, Cfg<1>::SMEM_BYTES, s>>>(m.a_hi, m.a_lo, m.b_hi, m.b_lo, p);
-      count_launch();
-      STK_CUDA(cudaGetLastError());
-    }
-    return 0;
-  }
+  const int CL = g_gemm_ctas == 2 && g_num_sms >= 2 ? 2 : 1;
   TcMaps m0, m1;
-  STK_TRY(make_maps(&m0, probs[0], nsplit, fp16, BN / 2));
+  STK_TRY(make_maps(&m0, probs[0], nsplit, fp16, BN / CL));
   auto mk_params = [&](const TcProblem& q) {
     GemmParams g{q.M, q.N, q.K, fp16, q.ep};
     g.conv_C = q.conv_C; g.conv_H = q.conv_H; g.conv_W = q.conv_W; g.conv_stride = q.conv_stride;
@@ -842,18 +478,15 @@ int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream
   GemmParams p1 = p0;
   p1.M = 0;
   m1 = m0;
-  int pairs = (int)((probs[0].M + 2 * BM - 1) / (2 * BM)) * ((probs[0].N + BN - 1) / BN);
+  int tiles = (int)((probs[0].M + CL * BM - 1) / (CL * BM)) * ((probs[0].N + BN - 1) / BN);
   if (n == 2) {
-    STK_TRY(make_maps(&m1, probs[1], nsplit, fp16, BN / 2));
+    STK_TRY(make_maps(&m1, probs[1], nsplit, fp16, BN / CL));
     p1 = mk_params(probs[1]);
-    pairs += (int)((probs[1].M + 2 * BM - 1) / (2 * BM)) * ((probs[1].N + BN - 1) / BN);
+    tiles += (int)((probs[1].M + CL * BM - 1) / (CL * BM)) * ((probs[1].N + BN - 1) / BN);
   }
-  const int clusters = pairs < g_num_sms / 2 ? pairs : g_num_sms / 2;
-  if (nsplit == 3) gemm_tc2_kernel<3><<<2 * clusters, NUM_THREADS, Cfg2<3>::SMEM_BYTES, s>>>(m0, m1, p0, p1);
-  else gemm_tc2_kernel<1><<<2 * clusters, NUM_THREADS, Cfg2<1>::SMEM_BYTES, s>>>(m0, m1, p0, p1);
-  count_launch();
-  STK_CUDA(cudaGetLastError());
-  return 0;
+  const int clusters = tiles < g_num_sms / CL ? tiles : g_num_sms / CL;
+  if (CL == 2) return launch_cl<2>(m0, m1, p0, p1, clusters, nsplit, fp16, s);
+  return launch_cl<1>(m0, m1, p0, p1, clusters, nsplit, fp16, s);
 }
 
 int launch_gemm_tc(const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, const __nv_bfloat16* W_hi,

@@ -6,7 +6,7 @@
 
 namespace stk {
 
-// Epilogue description common to the fp32-FFMA and the tcgen05 GEMMs:  y = act(A W^T + bias)
+// Epilogue description common to the fp32-FFMA and the tensor-core GEMMs:  y = act(A W^T + bias)
 //   mode EPI_STORE : out[orow, n] = y (+ addtab[(m % add_period) * add_ld + n])
 //   mode EPI_RESID : out[orow, n] = resid[orow, n] + gate[(m % gate_period) * gate_ld + n] * y   (gate NULL -> 1)
 //   mode EPI_SPLIT : out_hi/out_lo[orow, n] = bf16 split of y            (tensor-core A-operand planes)
@@ -90,7 +90,7 @@ int launch_bcast_rows(const float* src, const float* add, float* out, int B, int
 int launch_crop_pos(const float* pos, float* out, int max_size, int g, int D, cudaStream_t s);
 int launch_copy_rows(const float* src, int64_t src_bs, float* dst, int64_t dst_bs, int B, int64_t n_per_batch, cudaStream_t s);
 
-// ---- tcgen05 GEMM (gemm_tc.cu) --------------------------------------------------------------------------------
+// ---- wgmma GEMM (gemm_tc.cu) ----------------------------------------------------------------------------------
 // A planes [M,K] bf16 row-major (lo NULL iff nsplit == 1), W planes [N,K] bf16 row-major.
 // fp16 != 0: operands are IEEE half planes (nsplit must be 1).
 int launch_gemm_tc(const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, const __nv_bfloat16* W_hi,
@@ -105,14 +105,14 @@ struct TcProblem {
   // polyphase components of the input [images * 4, H_out, W_out, C] (pad right / bottom), conv_H / conv_W = output dims
   int conv_C = 0, conv_H = 0, conv_W = 0, conv_stride = 1;
 };
-// one launch for one or two independent problems of the same operand type (cta_group::2 kernel)
+// one launch for one or two independent problems of the same operand type
 int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream_t s, int fp16 = 0);
 int gemm_tc_init();   // resolves cuTensorMapEncodeTiled, sets smem attributes; idempotent
-void gemm_tc_set_ctas(int n);   // 2 (default): cta_group::2 pair kernel; 1: single-CTA kernel
+void gemm_tc_set_ctas(int n);   // 2 (default): two-CTA clusters sharing the W tile by TMA multicast; 1: one CTA per tile
 
 // ---- tensor-core attention -----------------------------------------------------------------------------------
 // qkv planes: packed 16-bit [B,S,3,H,64] (hi, and lo for the split mode), written by the QKV GEMM epilogue
-// tcgen05 / TMEM attention (attn_tc5.cu): single-pass 16-bit operands (fp16 != 0: IEEE half, else bf16), or -- with the lo
+// wgmma attention (attn_tc5.cu): single-pass 16-bit operands (fp16 != 0: IEEE half, else bf16), or -- with the lo
 // planes given -- the fp32-faithful split-bf16 mode (three MMAs per product, P split in registers)
 int launch_attention_tc5(const __nv_bfloat16* qkv16, int B, int S, int H, int ctx_rows, int ctx_keys, const AttnOut& out,
                          cudaStream_t s, int fp16, const __nv_bfloat16* qkv_lo = nullptr);

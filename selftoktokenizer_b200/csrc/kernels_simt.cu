@@ -1,6 +1,6 @@
-// fp32 FFMA kernels of the Selftok path (sm_100a): the encoder's fp32-faithful GEMMs and attention, the fused
+// fp32 FFMA kernels of the Selftok path (sm_90a): the encoder's fp32-faithful GEMMs and attention, the fused
 // VQ argmax, LayerNorm+modulate, and the small layout kernels.  These also serve as the bisecting reference for
-// the tcgen05 kernels (SELFTOK_PREC_FP32_SIMT).
+// the tensor-core kernels (SELFTOK_PREC_FP32_SIMT).
 //
 // Reference semantics restated here (file:line under /root/reference/mimogpt/models/selftok):
 //   linear  : nn.Linear everywhere (modules.py:147-162; sd3/mmdit.py:266-301; sd3/other_impls.py:82-84)
@@ -66,9 +66,8 @@ __global__ void __launch_bounds__(256, 2) linear_f32_kernel(const LinParams p) {
       Ws[buf][kq + 0][r] = rw[i].x; Ws[buf][kq + 1][r] = rw[i].y; Ws[buf][kq + 2][r] = rw[i].z; Ws[buf][kq + 3][r] = rw[i].w;
     }
   };
-  // accumulators as packed pairs (acc[i][2 j2], acc[i][2 j2 + 1]): the inner product runs on FFMA2 (fma.rn.f32x2: two independent
-  // round-to-nearest FMAs per issue slot, bit-identical to fmaf per element, same k order), which leaves every other issue slot
-  // to the shared-memory loads -- the scalar version spent all of them on FFMA and sat at half the FMA-pipe rate
+  // accumulators as packed pairs (acc[i][2 j2], acc[i][2 j2 + 1]) loaded straight from 64-bit shared-memory words; one
+  // round-to-nearest fmaf per element in a fixed k order, so the sums do not depend on the tile shape
   unsigned long long acc2[TM][TN / 2];
 #pragma unroll
   for (int i = 0; i < TM; ++i)
@@ -101,7 +100,7 @@ __global__ void __launch_bounds__(256, 2) linear_f32_kernel(const LinParams p) {
         unsigned long long ad;
         asm("mov.b64 %0, {%1, %1};" : "=l"(ad) : "f"(a[i]));
 #pragma unroll
-        for (int j = 0; j < TN / 2; ++j) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[i][j]) : "l"(ad), "l"(w2[j]));
+        for (int j = 0; j < TN / 2; ++j) fma2_packed(acc2[i][j], ad, w2[j]);
       }
     }
     if (kb + 1 < nk) {
@@ -290,7 +289,7 @@ int launch_ln_mod(const float* x, int64_t ldx, const float* shift, const float* 
 // Each CTA = 8 rows that share one shift / scale table row (staged in shared memory with cp.async under the x loads):
 // context problem position-major (the same position of 8 images), image problem natural order with its single per-step row.
 // One launch instead of two keeps the small late-schedule launches (B * Kc rows with Kc down to 20) from each leaving most
-// of the 148 SMs idle, and the output mode is compile-time (no per-element branches; one saturating F2FP per pair).
+// of the SMs idle, and the output mode is compile-time (no per-element branches; one saturating F2FP per pair).
 struct LnPairParams {
   LnProblem pr[2];
   int nblk0;               // CTAs of problem 0 (problem 1 owns the rest of the grid)
@@ -325,9 +324,7 @@ __global__ void __launch_bounds__(256) ln_mod_pair_kernel(const LnPairParams p) 
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   }
-  // All row arithmetic runs on the packed fp32 pipe (FADD2 / FFMA2, two elements per issue slot): under the 1 kW cap the SMs
-  // clock at ~1.35 GHz and this kernel is bound by instruction issue, not by HBM (91 % of the copy rate at burst clocks,
-  // 69 % in situ before this change).
+  // Row arithmetic on element pairs (fadd2 / ffma2: each lane rounded once, explicitly, so no contraction changes the sums).
 #pragma unroll 1
   for (int r = 0; r < ROWS; ++r) {
     const int64_t unit = first + 8 * r;
@@ -397,7 +394,10 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
   p.D = D; p.eps = eps;
   int nblk[2] = {0, 0};
   bool lo = false;
-  // two rows per warp when that still leaves >= 4 CTAs per SM of a B200 (halves the per-row share of the prologue); else one
+  // two rows per warp when that still leaves >= 4 CTAs per SM (halves the per-row share of the prologue); else one
+  int dev = 0, sms = 0;
+  STK_CUDA(cudaGetDevice(&dev));
+  STK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   auto ctas_for = [&](int rows_per_warp) {
     int64_t c = 0;
     for (int i = 0; i < n; ++i) {
@@ -407,7 +407,7 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
     }
     return c;
   };
-  const int rows = ctas_for(2) >= 4 * 148 ? 2 : 1;
+  const int rows = ctas_for(2) >= 4 * sms ? 2 : 1;
   for (int i = 0; i < 2; ++i) {
     if (i >= n) { p.pr[i] = probs[0]; p.pr[i].M = 0; continue; }
     LnProblem q = probs[i];
@@ -518,8 +518,7 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
     }
     __syncthreads();
     // ---- S = Q K^T (4 x 4 per thread)
-    // packed fp32 pipe (FFMA2: two independent round-to-nearest FMAs per issue slot, bit-identical to fmaf per element and in the
-    // same d order): accumulators as key pairs, the query element duplicated into both lanes
+    // accumulators as key pairs (one round-to-nearest fmaf per element, fixed d order), the query element duplicated into both lanes
     float sacc[4][4];
     {
       unsigned long long s2[4][2];
@@ -534,8 +533,8 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
         for (int i = 0; i < 4; ++i) {
           unsigned long long ad;
           asm("mov.b64 %0, {%1, %1};" : "=l"(ad) : "f"(av[i]));
-          asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(s2[i][0]) : "l"(ad), "l"(kk.x));
-          asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(s2[i][1]) : "l"(ad), "l"(kk.y));
+          fma2_packed(s2[i][0], ad, kk.x);
+          fma2_packed(s2[i][1], ad, kk.y);
         }
       }
 #pragma unroll
@@ -578,7 +577,7 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
     }
     __syncthreads();
     // ---- O += P V
-    if (DV % 2 == 0) {                                     // head dims 32 / 64: output-dim pairs on FFMA2, P duplicated
+    if (DV % 2 == 0) {                                     // head dims 32 / 64: output-dim pairs, P duplicated
       constexpr int DP = DV / 2 > 0 ? DV / 2 : 1;
       unsigned long long o2[4][DP];
 #pragma unroll
@@ -597,7 +596,7 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
           unsigned long long pd;
           asm("mov.b64 %0, {%1, %1};" : "=l"(pd) : "f"(pr[i]));
 #pragma unroll
-          for (int d = 0; d < DP; ++d) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(o2[i][d]) : "l"(pd), "l"(v2[d]));
+          for (int d = 0; d < DP; ++d) fma2_packed(o2[i][d], pd, v2[d]);
         }
       }
 #pragma unroll
@@ -775,9 +774,8 @@ __global__ void __launch_bounds__(256) vq_kernel(const float* __restrict__ z, in
     const int buf = ch & 1;
     if (ch + 1 < nch) { issue(ch + 1, buf ^ 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
     __syncthreads();
-    // scores of this thread's 4 rows x 8 codes as packed pairs (acc[i][2 j2], acc[i][2 j2 + 1]) on FFMA2 (fma.rn.f32x2: two
-    // independent round-to-nearest FMAs per issue slot, the same d order -> bit-identical to the scalar fmaf chain): the scalar
-    // version was issue-bound (ncu: issue 73 %, FMA pipe 51 %), the packed one leaves the slots to the LDS.128 and the argmax
+    // scores of this thread's 4 rows x 8 codes as packed pairs (acc[i][2 j2], acc[i][2 j2 + 1]), one round-to-nearest fmaf per
+    // element in a fixed d order -- the ids depend only on these sums
     unsigned long long acc2[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -793,7 +791,7 @@ __global__ void __launch_bounds__(256) vq_kernel(const float* __restrict__ z, in
         unsigned long long xd;
         asm("mov.b64 %0, {%1, %1};" : "=l"(xd) : "f"(xr[i][d]));
 #pragma unroll
-        for (int j = 0; j < 4; ++j) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[i][j]) : "l"(xd), "l"(cv2[j]));
+        for (int j = 0; j < 4; ++j) fma2_packed(acc2[i][j], xd, cv2[j]);
       }
     }
     float acc[4][8];

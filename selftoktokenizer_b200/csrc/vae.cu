@@ -9,7 +9,7 @@
 //   layout        NHWC.  The residual stream is fp32 [B, H, W, C]; every convolution / 1x1 projection reads its input as
 //                 16-bit operand planes (bf16 hi + lo: the fp32-faithful split mode, three MMAs per product) written by the
 //                 kernel that produces it (GroupNorm+SiLU, nearest upsample, softmax, GEMM epilogues).
-//   3x3 convs     implicit GEMM on the tcgen05 SM-pair kernel of gemm_tc.cu: A tile = 4-D TMA box of the NHWC planes shifted by
+//   3x3 convs     implicit GEMM on the wgmma kernel of gemm_tc.cu: A tile = 4-D TMA box of the NHWC planes shifted by
 //                 the tap offset (the TMA unit's out-of-bounds zero fill IS the padding), K = 9 C, weights repacked to
 //                 [Cout, (ky, kx), Cin]; bias and the residual add (x + h, ResnetBlock.forward :256) in the GEMM epilogue.
 //   stride-2 conv the input is written as its four polyphase planes (space_to_depth_planes_kernel); every tap is then a
@@ -17,7 +17,7 @@
 //   GroupNorm     32 groups, eps 1e-6, affine; two deterministic passes (per-chunk partial sums in a fixed order, then
 //                 normalise + SiLU + plane output) -- no atomics.
 //   attention     the single-head 512-channel block of the middle (AttnBlock.forward :276-287): per image S = Q K^T and
-//                 O = P V on the same tcgen05 GEMM (V^T comes straight out of its projection GEMM with the operands swapped; its
+//                 O = P V on the same wgmma GEMM (V^T comes straight out of its projection GEMM with the operands swapped; its
 //                 bias is added after P V, rows of P sum to one), row softmax in fp32.
 //
 // Weights under the reference's own SDVAE key names ("decoder.up.3.block.0.conv1.weight", ...).
@@ -206,7 +206,7 @@ __global__ void repack_conv_kernel(const float* __restrict__ w, float* __restric
   }
 }
 
-inline unsigned blocks_for(int64_t n, int per = 256, int64_t cap = 148 * 32) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + per - 1) / per, cap)); }
+inline unsigned blocks_for(int64_t n, int per = 256, int64_t cap = 132 * 32) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + per - 1) / per, cap)); }
 
 }  // namespace
 
@@ -254,8 +254,8 @@ extern "C" __attribute__((visibility("default"))) int selftok_vae_create(int ch,
   STK_CHECK(device >= 0 && device < ndev, SELFTOK_ERR_BAD_ARG, "bad device ordinal");
   cudaDeviceProp prop;
   STK_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device is not sm_100 (Blackwell B200): kernels are built for sm_100a only");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device is not sm_90 (Hopper H100): kernels are built for sm_90a only");
     return SELFTOK_ERR_NO_DEVICE;
   }
   STK_CUDA(cudaSetDevice(device));
@@ -414,8 +414,8 @@ static int vnorm(VaeCtx& c, const std::string& name, const float* x, int64_t HW,
   gn_finalize_kernel<<<c.B, 32, 0, c.s>>>(v->part, v->stats, nchunk, HW * (C / GN_GROUPS), 1e-6f);
   count_launch();
   const int64_t total4 = (int64_t)c.B * HW * (C / 4);
-  if (silu_act) gn_apply_kernel<true><<<blocks_for(total4, 256, 148 * 16), 256, 0, c.s>>>(x, v->stats, g, b, v->p_hi, v->p_lo, HW, C, total4);
-  else gn_apply_kernel<false><<<blocks_for(total4, 256, 148 * 16), 256, 0, c.s>>>(x, v->stats, g, b, v->p_hi, v->p_lo, HW, C, total4);
+  if (silu_act) gn_apply_kernel<true><<<blocks_for(total4, 256, 132 * 16), 256, 0, c.s>>>(x, v->stats, g, b, v->p_hi, v->p_lo, HW, C, total4);
+  else gn_apply_kernel<false><<<blocks_for(total4, 256, 132 * 16), 256, 0, c.s>>>(x, v->stats, g, b, v->p_hi, v->p_lo, HW, C, total4);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;
@@ -554,7 +554,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_vae_decode(selftok
       cin = cout;
     }
     if (lvl != 0) {
-      upsample2x_planes_kernel<<<blocks_for((int64_t)B * 4 * H * W * (cin / 4), 256, 148 * 16), 256, 0, s>>>(x, v->p_hi, v->p_lo, B, H, W, cin);
+      upsample2x_planes_kernel<<<blocks_for((int64_t)B * 4 * H * W * (cin / 4), 256, 132 * 16), 256, 0, s>>>(x, v->p_hi, v->p_lo, B, H, W, cin);
       count_launch();
       H *= 2; W *= 2;
       STK_TRY(vconv(c, "decoder.up." + std::to_string(lvl) + ".upsample.conv", v->p_hi, v->p_lo, H, W, y, nullptr));
@@ -595,7 +595,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_vae_encode(selftok
       cin = cout;
     }
     if (lvl != 3) {
-      space_to_depth_planes_kernel<<<blocks_for((int64_t)B * H * W * (cin / 4), 256, 148 * 16), 256, 0, s>>>(x, v->p_hi, v->p_lo, B, H, W, cin);
+      space_to_depth_planes_kernel<<<blocks_for((int64_t)B * H * W * (cin / 4), 256, 132 * 16), 256, 0, s>>>(x, v->p_hi, v->p_lo, B, H, W, cin);
       count_launch();
       H /= 2; W /= 2;
       STK_TRY(vconv(c, "encoder.down." + std::to_string(lvl) + ".downsample.conv", v->p_hi, v->p_lo, H, W, y, nullptr, 2));

@@ -12,7 +12,7 @@ GOLD = os.path.join(REPO, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100a) device; run with -m gpu on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90a, H100) device")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -65,7 +65,7 @@ def test_attention_f32(dev, B, Sq, S1, S2, H, hd):
 @pytest.mark.parametrize("nsplit", [3, 1, 0])
 @pytest.mark.parametrize("ctas", [2, 1])
 def test_gemm_tcgen05(dev, M, N, K, nsplit, ctas):
-    """tcgen05 GEMM (TMA + TMEM) vs fp64, both the cta_group::2 SM-pair kernel and the single-CTA kernel.
+    """Tensor-core GEMM (TMA + wgmma) vs fp64, both with two-CTA clusters sharing the W tile and with one CTA per tile.
     bf16x3 must be fp32-faithful; single-pass bf16 within bf16 rounding."""
     from selftoktokenizer_b200 import capi
     capi.k_set_gemm_ctas(ctas)
@@ -98,5 +98,5 @@ def test_attention_tensor_core(dev, B, S, H, ctx_rows, ctx_keys, nsplit):
         mask[:ctx_rows, ctx_keys:] = False
     ref = F.scaled_dot_product_attention(q, k, v, attn_mask=mask).transpose(1, 2).reshape(B, S, H * 64)
     err = (o.double() - ref).abs().max().item()
-    # tcgen05 + TMEM kernel: 3 = split bf16 (fp32-faithful), 1 = bf16, 0 = IEEE half
+    # wgmma kernel: 3 = split bf16 (fp32-faithful), 1 = bf16, 0 = IEEE half
     assert err < {3: 3e-5, 1: 2e-2, 0: 3e-3}[nsplit], err

@@ -1,5 +1,5 @@
 """Pins oracle/selftok_oracle.py (the CPU restatement) against the fixtures that oracle/gen_golden.py produced by
-running the UNMODIFIED reference modules, and — when /root/reference is mounted — against the live modules."""
+running the UNMODIFIED reference modules."""
 import dataclasses
 import os
 
@@ -108,24 +108,18 @@ def test_synthetic_weights_are_host_independent():
     assert abs(float(cb[0].norm(dim=-1).mean()) - 1.0) < 1e-6
 
 
-def test_live_reference_agrees_if_mounted(tiny_sd):
-    import ref_loader
-    if not ref_loader.reference_available():
-        pytest.skip("/root/reference not mounted (GPU box)")
-    ref_loader.import_reference()
-    enc_name, dit_name = ref_loader.register_geometry(C.TINY, "tinylive")
-    cfg = ref_loader.dims_to_cfg(C.TINY, enc_name, dit_name)
-    pipe = ref_loader.build_reference_pipeline(cfg, tiny_sd)
+def test_live_reference_agrees_if_mounted(tiny_sd, gold):
+    """The reference's own ImageTokenizer on the TINY geometry (tests/golden/tiny_live.npz, oracle/gen_golden.py tiny_live):
+    its state dict has every key of the spec with the same shape, and the restatement reproduces its encoder."""
+    g = gold("tiny_live")
+    ref_shapes = dict(zip(g["sd_keys"].tolist(), g["sd_shapes"].tolist()))
     # the state-dict contract: every key of the spec exists in the reference module with the same shape
-    ref_sd = pipe.model.state_dict()
     for name, (shape, _, _) in synth.state_dict_spec(C.TINY).items():
-        assert name in ref_sd and tuple(ref_sd[name].shape) == tuple(shape), name
+        assert name in ref_shapes and ref_shapes[name] == "x".join(str(n) for n in shape), name
     x0 = synth.synth_tensor("live.x0", (2, 16, 8, 8), "emb", 1.0)
-    with torch.no_grad():
-        outs_q_ref, tok_ref = pipe.model.encoder(x0, d=None)
     outs_q, tok, _ = O.encode(tiny_sd, C.TINY, x0)
-    assert torch.equal(tok, tok_ref)
-    assert (outs_q - outs_q_ref).abs().max() < 1e-5
+    assert torch.equal(tok, torch.from_numpy(g["tokens"]))
+    assert (outs_q - torch.from_numpy(g["outs_q"])).abs().max() < 1e-5
 
 
 # ------------------------------------------------------------------ plain-C restatement of the index path (oracle/vq_oracle.c)
@@ -230,12 +224,14 @@ def test_pixel_fixture_is_reference_latents_through_the_vae_oracle(gold):
     assert np.abs(px.numpy() - gp["pixels"]).max() < 2e-5
 
 
-def test_boundary_helpers_match_the_live_reference():
+def test_boundary_helpers_match_the_live_reference(gold):
     """a13: NormalizeToTensor, norm_ip, SD3LatentFormat against the reference's own definitions
-    (SelftokPipeline.py:85-97,135-137; sd3/sd3_impls.py:133-144)."""
+    (SelftokPipeline.py:85-97,135-137; sd3/sd3_impls.py:133-144), as recorded in tests/golden/boundary_helpers.npz."""
     from selftoktokenizer_b200 import pipeline as P
+    g = gold("boundary_helpers")
     rng = np.random.RandomState(0)
     img = rng.randint(0, 256, size=(24, 40, 3)).astype(np.uint8)
+    assert np.array_equal(img, g["img"])
     t = P.NormalizeToTensor()(img)
     assert t.shape == (3, 24, 40) and t.dtype == torch.float32
     assert float(t.min()) >= -1.0 and float(t.max()) <= 1.0
@@ -246,21 +242,14 @@ def test_boundary_helpers_match_the_live_reference():
     y = x.clone()
     P.norm_ip(y, -1, 1)
     assert torch.equal(y, torch.tensor([0.0, 0.0, 0.5, 0.75, 1.0, 1.0]))
-    lat = torch.randn(2, 16, 4, 4)
+    lat = torch.from_numpy(g["lat"])
     f = P.SD3LatentFormat()
     assert torch.allclose(f.process_out(f.process_in(lat)), lat, atol=1e-6)
     assert torch.equal(f.process_in(lat), (lat - 0.0609) * 1.5305)
-    import ref_loader
-    if not ref_loader.reference_available():
-        return
-    ref_loader.import_reference()
-    from mimogpt.infer import SelftokPipeline as SP
-    from mimogpt.models.selftok.sd3.sd3_impls import SD3LatentFormat as RefFmt
-    assert torch.equal(SP.NormalizeToTensor()(img), t)
-    y2 = x.clone()
-    SP.norm_ip(y2, -1, 1)
-    assert torch.equal(y2, y)
-    assert torch.equal(RefFmt().process_in(lat), f.process_in(lat)) and torch.equal(RefFmt().process_out(lat), f.process_out(lat))
+    # the reference's own outputs on the same inputs
+    assert torch.equal(torch.from_numpy(g["normalized"]), t)
+    assert torch.equal(torch.from_numpy(g["x"]), x) and torch.equal(torch.from_numpy(g["norm_ip"]), y)
+    assert torch.equal(torch.from_numpy(g["lat_in"]), f.process_in(lat)) and torch.equal(torch.from_numpy(g["lat_out"]), f.process_out(lat))
 
 
 def test_ema_decoder_state_selection():

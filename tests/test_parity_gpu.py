@@ -376,7 +376,7 @@ def test_full_pixel_gate(full_engine, gold):
 def test_full_renderer_pixel_gate(gold):
     import vae_oracle as V
     from selftoktokenizer_b200.capi import Engine
-    gr, ge, gp = gold("full_renderer"), gold("full_encode"), gold("full_pixels")
+    gr, ge, gp = gold("full_renderer"), gold("full_encode"), gold("full_renderer_pixels")
     d = dataclasses.replace(C.FULL, renderer=True)
     vsd = synth.synth_vae_state_dict(ch=128, encoder=False)
     eng = Engine(d, synth.synth_state_dict(d, device=DEV), device=DEV, precision="auto")
@@ -387,7 +387,7 @@ def test_full_renderer_pixel_gate(gold):
         px = V.images_from_latents(vsd, r).numpy()
         x0 = synth.synth_tensor("golden.full.x0", (2, d.in_channels, d.latent, d.latent), "emb", 1.0)[:1]
         gt = V.images_from_latents(vsd, x0).numpy()
-    _pixel_gate(px, gp["renderer_pixels"], gt, "full renderer bf16x3")
+    _pixel_gate(px, gp["pixels"], gt, "full renderer bf16x3")
 
 
 @pytest.mark.parametrize("fixture,stress", [("mid", False), ("mid_stress", True)])
@@ -578,7 +578,7 @@ def test_guided_sampler_cfg(tiny_engine, gold):
 
 @pytest.mark.parametrize("h,B", [(8, 3), (16, 2), (32, 2)])
 def test_device_vae_decoder_against_oracle(h, B):
-    """f1: the SD3 VAE decoder on the device (implicit-GEMM 3x3 convolutions on the tcgen05 kernel, GroupNorm + SiLU, the
+    """f1: the SD3 VAE decoder on the device (implicit-GEMM 3x3 convolutions on the wgmma kernel, GroupNorm + SiLU, the
     single-head attention of the middle block) against the pinned restatement of the reference's SDVAE, seeded weights."""
     import vae_oracle as V
     from selftoktokenizer_b200.capi import VaeDecoder
