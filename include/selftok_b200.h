@@ -143,6 +143,28 @@ int selftok_dit_velocity(selftok_handle_t h, const int64_t* tokens_dev, const fl
 /* renderer handles only: tokens_dev [B,K] -> pred_x0 [B,C,latent,latent]. */
 int selftok_render(selftok_handle_t h, const int64_t* tokens_dev, int B, float* x0_out_dev, void* stream);
 
+/* ---- token ranges: decode part of each image's token sequence ----------------------------------------------
+ * range_host: host int32 [B][2] of (lo_b, hi_b) windows, 0 <= lo_b < hi_b <= K.  Image b is decoded from its ids [lo_b, hi_b)
+ * only: ids outside the window are not read, not validated and not counted by selftok_id_errors (pad with anything, e.g. -1);
+ * ids inside follow the usual rules.  Selftok sequences are autoregressive and consumed in reverse index order, so n generated
+ * tokens are the window (K - n, K) and a truncated prefix is (0, n).
+ *   sampler     at step i the visible tokens are [lo_b, min(hi_b, k_i + 1)) -- the reference's p_sample_loop(..., super_mask)
+ *               (sd3/rectified_flow.py:182,227-231); the window may be empty at late steps (image stream without context keys)
+ *   guided      the same mask is the conditional branch's mask (rectified_flow.py:281-288); every window must keep a visible
+ *               token at every executed step (lo_b <= k_{steps-1}), else SELFTOK_ERR_BAD_ARG (the reference is NaN there)
+ *   renderer    MMDiT_Renderer.forward(..., mask = the window) (sd3/mmdit.py:1529,1562-1614), no schedule clipping
+ * A bad window returns SELFTOK_ERR_BAD_ARG before any launch; selftok_last_error() names the image.  An image's result depends
+ * only on its ids inside its window, its noise and its window (bitwise the same alone or in any batch); [0, K) for every image
+ * is bitwise selftok_decode / selftok_decode_cfg / selftok_render.  The batch's windows are rounded outward to 64 tokens
+ * ([Lo, Hi)): the context stream covers those positions, and one CUDA graph per (B, steps, Lo, Hi) serves every range set
+ * with the same rounding.  The per-call plan lives in the decode workspace (counted by selftok_workspace_bytes). */
+int selftok_decode_range(selftok_handle_t h, const int64_t* tokens_dev, const int32_t* range_host, const float* noise_dev,
+                         int B, int steps, float* x0_out_dev, void* stream);
+int selftok_decode_cfg_range(selftok_handle_t h, const int64_t* tokens_dev, const int32_t* range_host, const float* noise_dev,
+                             int B, int steps, float cfg_scale, float* x0_out_dev, void* stream);
+int selftok_render_range(selftok_handle_t h, const int64_t* tokens_dev, const int32_t* range_host, int B, float* x0_out_dev,
+                         void* stream);
+
 /* ---- hot path, host buffers (what SelftokPipeline's numpy-in / tensor-out API maps to; H2D and D2H copies are
  * inside the call, on `stream`, followed by a stream synchronize) --------------------------------------------- */
 int selftok_encode_host(selftok_handle_t h, const float* x0_host, int B, int64_t* tokens_host, void* stream);
@@ -220,6 +242,12 @@ int selftok_k_attention_f32(const float* q_dev, int64_t q_ld, const float* k1_de
  * nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass. */
 int selftok_k_attention_tc(const float* qkv_dev, float* out_dev, int B, int S, int H, int nsplit,
                            int ctx_rows, int ctx_keys, void* stream);
+/* The same attention with per-image live context counts (the layout of a token-range call): live_host is host int32 [1 + B] =
+ * {Kc, c_0, ..., c_{B-1}}.  Rows [0, c_b) of image b are its live context rows, [c_b, c_b + S - Kc) its image rows, the rest
+ * context rows outside the window.  Image rows see keys [0, c_b + S - Kc); context rows the same, or [0, c_b) with ctx_self != 0;
+ * a row with no visible key writes 0.  out_dev [B,S,H*64] in row order. */
+int selftok_k_attention_tc_range(const float* qkv_dev, float* out_dev, int B, int S, int H, int nsplit, int ctx_self,
+                                 const int32_t* live_host, void* stream);
 
 #ifdef __cplusplus
 }

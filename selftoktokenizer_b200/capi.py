@@ -26,7 +26,7 @@ SYMBOLS = [
     "selftok_set_cfg_schedule", "selftok_decode", "selftok_decode_cfg", "selftok_dit_velocity", "selftok_render", "selftok_encode_host", "selftok_decode_host",
     "selftok_render_host", "selftok_id_errors", "selftok_workspace_bytes", "selftok_set_workspace", "selftok_last_launch_count", "selftok_device_bytes", "selftok_set_use_graph",
     "selftok_set_profile", "selftok_get_profile", "selftok_k_linear_f32", "selftok_k_linear_tc", "selftok_k_set_gemm_ctas", "selftok_k_ln_mod_f32", "selftok_k_attention_f32",
-    "selftok_k_attention_tc",
+    "selftok_k_attention_tc", "selftok_decode_range", "selftok_decode_cfg_range", "selftok_render_range", "selftok_k_attention_tc_range",
     "selftok_vae_create", "selftok_vae_destroy", "selftok_vae_load_tensor", "selftok_vae_finalize", "selftok_vae_decode", "selftok_vae_encode", "selftok_vae_device_bytes",
 ]
 
@@ -94,6 +94,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.selftok_k_ln_mod_f32.argtypes = [vp, vp, vp, i64, i32, vp, i64, i32, vp]
     lib.selftok_k_attention_f32.argtypes = [vp, i64, vp, vp, i64, i32, vp, vp, i64, i32, vp, i64, i32, i32, i32, i32, vp]
     lib.selftok_k_attention_tc.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    lib.selftok_decode_range.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp]
+    lib.selftok_decode_cfg_range.argtypes = [vp, vp, vp, vp, i32, i32, C.c_float, vp, vp]
+    lib.selftok_render_range.argtypes = [vp, vp, vp, i32, vp, vp]
+    lib.selftok_k_attention_tc_range.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp]
     lib.selftok_vae_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.selftok_vae_destroy.argtypes = [vp]
     lib.selftok_vae_load_tensor.argtypes = [vp, C.c_char_p, vp, i32, C.POINTER(i64), i32]
@@ -262,14 +266,23 @@ class Engine:
             raise SelftokError(f"{what}: expected [B, {want[0]}, {want[1]}, {want[2]}] latents for this engine "
                                f"(image side {8 * d.latent}), got {tuple(x.shape)}")
 
-    def _check_tokens(self, tokens: torch.Tensor, what: str, batch: Optional[int] = None, is_output: bool = False) -> None:
+    def _check_tokens(self, tokens: torch.Tensor, what: str, batch: Optional[int] = None, is_output: bool = False,
+                      ranges: Optional[np.ndarray] = None) -> None:
         if tokens.dim() != 2 or tokens.shape[1] != self.dims.K or tokens.shape[0] < 1:
             raise SelftokError(f"{what}: expected [B, {self.dims.K}] token ids, got {tuple(tokens.shape)}")
         if batch is not None and tokens.shape[0] != batch:
             raise SelftokError(f"{what}: {tokens.shape[0]} token rows for a batch of {batch}")
         if not tokens.is_cuda and not is_output:
             # ids outside the codebook are an error in the reference (`codebook[idx]` raises).  Host tensors are checked here
-            # for free; device tensors are checked by the kernel (NaN rows + counter, see `id_errors`).
+            # for free; device tensors are checked by the kernel (NaN rows + counter, see `id_errors`).  With token ranges only
+            # the ids inside each image's window are read, so only those are checked.
+            if ranges is not None:
+                pos = torch.arange(self.dims.K)
+                r = torch.from_numpy(ranges).long()
+                inside = (pos[None] >= r[:, :1]) & (pos[None] < r[:, 1:])
+                if not bool(inside.any()):
+                    return
+                tokens = tokens[inside]
             lo, hi = int(tokens.min()), int(tokens.max())
             if lo < 0 or hi >= self.dims.codebook_size:
                 raise SelftokError(f"{what}: token id out of range [0, {self.dims.codebook_size}): min {lo}, max {hi}")
@@ -314,28 +327,53 @@ class Engine:
             check(self.lib.selftok_lookup(self.h, tokens.data_ptr(), B, out.data_ptr(), _stream_ptr(self.device)))
         return out
 
-    def decode(self, tokens: torch.Tensor, noise: torch.Tensor, steps: Optional[int] = None) -> torch.Tensor:
+    @staticmethod
+    def token_ranges(token_range, B: int) -> np.ndarray:
+        """`token_range` -> contiguous int32 [B, 2] (lo, hi) windows: a (lo, hi) pair for the whole batch or an int array [B, 2].
+        The windows themselves (0 <= lo < hi <= K) are validated by the library."""
+        r = np.asarray(token_range)
+        if r.shape == (2,):
+            r = np.broadcast_to(r, (B, 2))
+        if r.shape != (B, 2) or not np.issubdtype(r.dtype, np.integer):
+            raise SelftokError(f"token_range: expected a (lo, hi) pair or an int array [{B}, 2], got {r.dtype} {r.shape}")
+        return np.ascontiguousarray(r, dtype=np.int32)
+
+    def decode(self, tokens: torch.Tensor, noise: torch.Tensor, steps: Optional[int] = None, *, token_range=None) -> torch.Tensor:
+        """tokens [B,K], noise [B,C,h,w] -> latents after `steps` Euler steps.  token_range (see `token_ranges`): image b is decoded
+        from its ids [lo_b, hi_b) only (selftok_decode_range); n generated tokens of the AR order = (K - n, K)."""
         self._check_latent(noise, "decode (noise)")
-        self._check_tokens(tokens, "decode", noise.shape[0])
+        rng = None if token_range is None else self.token_ranges(token_range, noise.shape[0])
+        self._check_tokens(tokens, "decode", noise.shape[0], ranges=rng)
         tokens = self._dev(tokens, torch.int64)
         noise = self._dev(noise, torch.float32)
         B = tokens.shape[0]
         out = torch.empty_like(noise)
         with torch.cuda.device(self.device):
-            check(self.lib.selftok_decode(self.h, tokens.data_ptr(), noise.data_ptr(), B, steps or self.steps,
-                                          out.data_ptr(), _stream_ptr(self.device)))
+            if rng is None:
+                check(self.lib.selftok_decode(self.h, tokens.data_ptr(), noise.data_ptr(), B, steps or self.steps,
+                                              out.data_ptr(), _stream_ptr(self.device)))
+            else:
+                check(self.lib.selftok_decode_range(self.h, tokens.data_ptr(), rng.ctypes.data, noise.data_ptr(), B, steps or self.steps,
+                                                    out.data_ptr(), _stream_ptr(self.device)))
         return out
 
-    def decode_cfg(self, tokens: torch.Tensor, noise: torch.Tensor, cfg_scale: float, steps: Optional[int] = None) -> torch.Tensor:
-        """Guided sampler: the reference's p_sample_loop(..., uncond_scale=cfg_scale) (rectified_flow.py:280-289)."""
+    def decode_cfg(self, tokens: torch.Tensor, noise: torch.Tensor, cfg_scale: float, steps: Optional[int] = None, *,
+                   token_range=None) -> torch.Tensor:
+        """Guided sampler: the reference's p_sample_loop(..., uncond_scale=cfg_scale) (rectified_flow.py:280-289).  token_range as
+        in `decode`; every window must keep a visible token at the last executed step (lo <= k of that step)."""
         self._check_latent(noise, "decode_cfg (noise)")
-        self._check_tokens(tokens, "decode_cfg", noise.shape[0])
+        rng = None if token_range is None else self.token_ranges(token_range, noise.shape[0])
+        self._check_tokens(tokens, "decode_cfg", noise.shape[0], ranges=rng)
         tokens = self._dev(tokens, torch.int64)
         noise = self._dev(noise, torch.float32)
         out = torch.empty_like(noise)
         with torch.cuda.device(self.device):
-            check(self.lib.selftok_decode_cfg(self.h, tokens.data_ptr(), noise.data_ptr(), tokens.shape[0], steps or self.steps,
-                                              float(cfg_scale), out.data_ptr(), _stream_ptr(self.device)))
+            if rng is None:
+                check(self.lib.selftok_decode_cfg(self.h, tokens.data_ptr(), noise.data_ptr(), tokens.shape[0], steps or self.steps,
+                                                  float(cfg_scale), out.data_ptr(), _stream_ptr(self.device)))
+            else:
+                check(self.lib.selftok_decode_cfg_range(self.h, tokens.data_ptr(), rng.ctypes.data, noise.data_ptr(), tokens.shape[0],
+                                                        steps or self.steps, float(cfg_scale), out.data_ptr(), _stream_ptr(self.device)))
         return out
 
     def dit_velocity(self, tokens: torch.Tensor, x: torch.Tensor, step: int) -> torch.Tensor:
@@ -349,13 +387,19 @@ class Engine:
                                                 out.data_ptr(), _stream_ptr(self.device)))
         return out
 
-    def render(self, tokens: torch.Tensor) -> torch.Tensor:
-        self._check_tokens(tokens, "render")
+    def render(self, tokens: torch.Tensor, *, token_range=None) -> torch.Tensor:
+        """Renderer pass; token_range as in `decode` (the window is the renderer's mask, selftok_render_range)."""
+        rng = None if token_range is None or tokens.dim() != 2 else self.token_ranges(token_range, tokens.shape[0])
+        self._check_tokens(tokens, "render", ranges=rng)
         tokens = self._dev(tokens, torch.int64)
         d = self.dims
         out = torch.empty(tokens.shape[0], d.in_channels, d.latent, d.latent, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            check(self.lib.selftok_render(self.h, tokens.data_ptr(), tokens.shape[0], out.data_ptr(), _stream_ptr(self.device)))
+            if rng is None:
+                check(self.lib.selftok_render(self.h, tokens.data_ptr(), tokens.shape[0], out.data_ptr(), _stream_ptr(self.device)))
+            else:
+                check(self.lib.selftok_render_range(self.h, tokens.data_ptr(), rng.ctypes.data, tokens.shape[0], out.data_ptr(),
+                                                    _stream_ptr(self.device)))
         return out
 
     # ------------------------------------------------------------------ hot path (host buffers; copies inside the call)
@@ -586,6 +630,17 @@ def k_attention_f32(q, k1, v1, k2=None, v2=None, heads=1):
     out = torch.empty_like(q)
     check(lib.selftok_k_attention_f32(q.data_ptr(), Dm, k1.data_ptr(), v1.data_ptr(), Dm, S1, _ptr(k2), _ptr(v2), Dm, S2,
                                       out.data_ptr(), Dm, B, Sq, heads, Dm // heads, _stream_ptr(q.device)))
+    return out
+
+
+def k_attention_tc_range(qkv, heads, Kc, live, nsplit=3, ctx_self=False):
+    """qkv [B,S,3,H,64] fp32, Kc context rows per slot, live [B] live context rows per image -> [B,S,H*64] (slot row order)."""
+    lib = load_library()
+    B, S = qkv.shape[0], qkv.shape[1]
+    arr = np.ascontiguousarray([Kc, *[int(c) for c in live]], dtype=np.int32)
+    out = torch.empty(B, S, heads * 64, dtype=torch.float32, device=qkv.device)
+    check(lib.selftok_k_attention_tc_range(qkv.data_ptr(), out.data_ptr(), B, S, heads, nsplit, int(ctx_self), arr.ctypes.data,
+                                           _stream_ptr(qkv.device)))
     return out
 
 

@@ -12,7 +12,9 @@
 //   epilogue       O / l -> fp32 and / or the 16-bit A-operand planes of the proj GEMM
 //
 // Contract (sd3/mmdit.py:521-531, sd3/other_impls.py:37-45): dense non-causal attention over the joint
-// [context prefix ; image] sequence; rows < ctx_rows only see keys < ctx_keys (renderer rule, mmdit.py:1581).
+// [context prefix ; image] sequence; rows < ctx_rows only see keys < ctx_keys (renderer rule, mmdit.py:1581).  With a
+// token-range plan (AttnPlan) every image has its own number of live context rows and keys; the key loop of the producer and of
+// the consumers stops at the image's last visible key.
 #include "common.cuh"
 #include "hopper.cuh"
 #include "kernels.h"
@@ -74,6 +76,7 @@ struct Attn5Params {
   AttnOut out;
   int B, S, H, ctx_rows, ctx_keys, fp16;
   float scale_log2e;
+  AttnPlan pl;
 };
 
 template <bool FP16, int NSPLIT>
@@ -97,7 +100,10 @@ attention_tc5_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
   const int nq = (S + BQ - 1) / BQ;
   const int item = blockIdx.x;
   const int qt = item % nq, h = (item / nq) % p.H, b = item / (nq * p.H);
-  const int kmax_cta = ((qt + 1) * BQ <= p.ctx_rows) ? p.ctx_keys : S;   // every row of the tile is a context row
+  // token-range plan: this image's live context rows pc and live keys [0, live); a tile of context rows only stops at pc
+  const int pc = p.pl.plan ? p.pl.plan[2 * b + 1] : 0, live = p.pl.plan ? pc + p.pl.n_img : S;
+  const int kmax_cta = !p.pl.plan ? (((qt + 1) * BQ <= p.ctx_rows) ? p.ctx_keys : S)   // every row of the tile is a context row
+                                  : ((p.pl.ctx_self && ((qt + 1) * BQ <= pc || qt * BQ >= live)) ? pc : live);
   const int n_tiles = (kmax_cta + BKV - 1) / BKV;
   const int row0 = b * S;                                     // first row of this image in the [B*S, 3*H*64] matrix
 
@@ -138,7 +144,10 @@ attention_tc5_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
   const int rt = wg * 64 + (wl >> 5) * 16 + (lane >> 2);
   int kmax[2];
 #pragma unroll
-  for (int r = 0; r < 2; ++r) kmax[r] = (qt * BQ + rt + 8 * r < p.ctx_rows) ? p.ctx_keys : S;
+  for (int r = 0; r < 2; ++r) {
+    const int row = qt * BQ + rt + 8 * r;
+    kmax[r] = !p.pl.plan ? ((row < p.ctx_rows) ? p.ctx_keys : S) : ((p.pl.ctx_self && (row < pc || row >= live)) ? pc : live);
+  }
   float m_run[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};
   float o[32];
 #pragma unroll
@@ -224,9 +233,13 @@ attention_tc5_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const int row = qt * BQ + rt + 8 * r;
     if (row >= S) continue;
-    const float inv = 1.0f / l;
-    const bool inA = row < t.split;
-    const int64_t orow = inA ? ((int64_t)b * t.split + row) : ((int64_t)b * (S - t.split) + (row - t.split));
+    const float inv = l > 0.f ? 1.0f / l : 0.f;                // a row with no visible key (token-range plan) writes 0
+    bool inA = row < t.split;
+    int64_t orow = inA ? ((int64_t)b * t.split + row) : ((int64_t)b * (S - t.split) + (row - t.split));
+    if (p.pl.plan && p.pl.route) {
+      const int sr = plan_stream_row(row, p.pl.plan[2 * b], pc, p.pl.n_img, inA);
+      orow = inA ? (int64_t)b * t.split + sr : (int64_t)b * p.pl.n_img + sr;
+    }
     float* of = inA ? t.f32_a : t.f32_b;
     __nv_bfloat16* oh = inA ? t.hi_a : t.hi_b;
     __nv_bfloat16* ol = inA ? t.lo_a : t.lo_b;
@@ -249,11 +262,13 @@ bool g_attr_dev[64];       // cudaFuncSetAttribute is per device: one handle per
 }  // namespace
 
 int launch_attention_tc5(const __nv_bfloat16* qkv16, int B, int S, int H, int ctx_rows, int ctx_keys, const AttnOut& out,
-                         cudaStream_t s, int fp16, const __nv_bfloat16* qkv_lo) {
+                         cudaStream_t s, int fp16, const __nv_bfloat16* qkv_lo, const AttnPlan& plan) {
   STK_CHECK(qkv16 && B > 0 && S > 0 && H > 0, -1, "attention_tc5: bad arguments");
   STK_CHECK(out.ld % 8 == 0, -1, "attention_tc5: output pitch must be a multiple of 8");
   STK_CHECK(ctx_keys <= S && ctx_rows <= S && ctx_keys >= 0 && ctx_rows >= 0, -1, "attention_tc5: context limits exceed the sequence");
   STK_CHECK(!(fp16 && qkv_lo), -1, "attention_tc5: the split mode uses bf16 planes");
+  STK_CHECK(!plan.plan || (plan.n_img > 0 && plan.n_img <= S && (!plan.route || out.split == S - plan.n_img)), -1,
+            "attention_tc5: inconsistent token-range plan");
   STK_TRY(gemm_tc_init());
   int dev = 0;
   STK_CUDA(cudaGetDevice(&dev));
@@ -273,7 +288,7 @@ int launch_attention_tc5(const __nv_bfloat16* qkv16, int B, int S, int H, int ct
     STK_TRY(make_tensor_map_2d(&mql, qkv_lo, rows, cols, BQ, HD, 0));
     STK_TRY(make_tensor_map_2d(&mkvl, qkv_lo, rows, cols, BKV, HD, 0));
   }
-  Attn5Params p{out, B, S, H, ctx_rows, ctx_keys, fp16, 0.125f * 1.4426950408889634f};
+  Attn5Params p{out, B, S, H, ctx_rows, ctx_keys, fp16, 0.125f * 1.4426950408889634f, plan};
   const int n_items = ((S + BQ - 1) / BQ) * H * B;
   if (qkv_lo) attention_tc5_kernel<false, 3><<<n_items, NUM_THREADS, A5<3>::SMEM_BYTES, s>>>(mq, mkv, mql, mkvl, p);
   else if (fp16) attention_tc5_kernel<true, 1><<<n_items, NUM_THREADS, A5<1>::SMEM_BYTES, s>>>(mq, mkv, mql, mkvl, p);

@@ -13,6 +13,7 @@
 #include <string.h>
 #include <map>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -68,6 +69,7 @@ struct DecodeWs {       // activation workspace of the MMDiT for one batch size
   bf16 *a_c_hi = nullptr, *a_c_lo = nullptr, *a_x_hi = nullptr, *a_x_lo = nullptr;
   bf16 *attn_c_hi = nullptr, *attn_c_lo = nullptr, *attn_x_hi = nullptr, *attn_x_lo = nullptr;
   bf16 *h_c_hi = nullptr, *h_c_lo = nullptr, *h_x_hi = nullptr, *h_x_lo = nullptr;
+  int* plan = nullptr;                           // token-range calls: [B][2] windows (lo, hi), then the plan [steps][B][2] (a, c)
   void* own = nullptr;                           // the library's own block (NULL when the caller's workspace is in use)
   size_t own_bytes = 0;
 };
@@ -107,6 +109,11 @@ struct selftok_engine {
   void* user_ws[2] = {nullptr, nullptr};          // caller-provided workspaces (selftok_set_workspace): [0] encode, [1] decode / render
   size_t user_ws_bytes[2] = {0, 0};
   std::map<std::pair<int, int>, std::pair<cudaGraphExec_t, int64_t>> graphs;   // (B, steps) -> (exec, launches)
+  std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, int64_t>> range_graphs;   // token ranges: (B, steps, Lo, Hi)
+  std::vector<int> plan_host;           // token-range plan of the current call, built on the host
+  int* plan_pinned = nullptr;           // pinned staging copy of it (an H2D copy from pageable memory would block the host)
+  size_t plan_pinned_n = 0;
+  cudaEvent_t plan_copied = nullptr;    // recorded after each upload: the staging buffer is reused only once it has completed
   std::map<int, std::pair<cudaGraphExec_t, int64_t>> enc_graphs;               // encode, B -> (exec, launches)
   int64_t last_launches = 0;
   // optional per-kernel-class timing (CUDA events around every launch; only meaningful with graphs disabled)
@@ -276,6 +283,9 @@ extern "C" __attribute__((visibility("default"))) int selftok_destroy(selftok_ha
   cudaSetDevice(e->cfg.device);
   cudaDeviceSynchronize();
   for (auto& g : e->graphs) cudaGraphExecDestroy(g.second.first);
+  for (auto& g : e->range_graphs) cudaGraphExecDestroy(g.second.first);
+  if (e->plan_pinned) cudaFreeHost(e->plan_pinned);
+  if (e->plan_copied) cudaEventDestroy(e->plan_copied);
   for (auto& kv : e->w) cudaFree(kv.second.d);
   free_pool(e, e->allocs);
   if (e->bad_ids) cudaFree(e->bad_ids);
@@ -840,12 +850,13 @@ extern "C" __attribute__((visibility("default"))) int selftok_vq_argmax(selftok_
   return SELFTOK_OK;
 }
 
-static int run_lookup(selftok_engine* e, const int64_t* tokens, int B, float* outs_q, cudaStream_t s) {
+// range != NULL: device [B][2] token windows; ids outside an image's window are not read (zero rows)
+static int run_lookup(selftok_engine* e, const int64_t* tokens, int B, float* outs_q, cudaStream_t s, const int* range = nullptr) {
   GETW(cb, "encoder.quantizer._codebook.embed");
   GETW(lw, "encoder.final_layer_norm3.weight");
   GETW(lb, "encoder.final_layer_norm3.bias");
   PROF(PC_OTHER, launch_lookup_ln3(tokens, (int64_t)B * e->cfg.K, cb->d, e->cfg.codebook_size, e->cfg.code_dim, lw->d, lb->d, outs_q,
-                                   e->bad_ids, s));
+                                   e->bad_ids, s, range, e->cfg.K));
   return 0;
 }
 
@@ -893,6 +904,7 @@ static int layout_dws(selftok_engine* e, DecodeWs& w, int64_t B, Arena& A) {
   STK_TRY(A.take(&w.o_final, B * N * c.dit_patch * c.dit_patch * c.in_channels));
   STK_TRY(A.take(&w.o_final_u, B * N * c.dit_patch * c.dit_patch * c.in_channels));
   STK_TRY(A.take(&w.a_x, B * N * D));                       // fp32 LN output of the final layer (both modes)
+  STK_TRY(A.take(&w.plan, B * 2 * (1 + (int64_t)e->steps)));
   if (!tc_mode(e)) {
     STK_TRY(A.take(&w.qkv, B * S * 3 * D));
     STK_TRY(A.take(&w.a_c, B * K * D));
@@ -925,10 +937,15 @@ static int layout_dws(selftok_engine* e, DecodeWs& w, int64_t B, Arena& A) {
   }
   return 0;
 }
+static void drop_decode_graphs(selftok_engine* e) {
+  for (auto& g : e->graphs) cudaGraphExecDestroy(g.second.first);
+  e->graphs.clear();
+  for (auto& g : e->range_graphs) cudaGraphExecDestroy(g.second.first);
+  e->range_graphs.clear();
+}
 static int ensure_dws(selftok_engine* e, int B) {
   if (e->dws.B >= B) return 0;
-  for (auto& g : e->graphs) cudaGraphExecDestroy(g.second.first);   // graphs hold pointers into the old workspace
-  e->graphs.clear();
+  drop_decode_graphs(e);                                            // graphs hold pointers into the old workspace
   free_dws(e);
   return place_ws(e, 1, e->dws, B, [&](DecodeWs& w, int64_t b, Arena& A) { return layout_dws(e, w, b, A); });
 }
@@ -936,11 +953,12 @@ static int ensure_dws(selftok_engine* e, int B) {
 // One stream of one JointBlock: LN+modulate -> qkv GEMM into the joint buffer   (mmdit.py:441-483, 521-529)
 static int pre_attention(selftok_engine* e, const std::string& blk, const float* resid, int64_t M, const float* shift,
                          const float* scale, int64_t ld_mod, int period, float* a32, bf16* a_hi, bf16* a_lo, int rpb_in,
-                         int S, int row_off, cudaStream_t s) {
+                         int S, int row_off, cudaStream_t s, const int* plan = nullptr, int plan_ctx = 0) {
   const int D = e->D;
   DecodeWs& w = e->dws;
   Epilogue ep;
   ep.out = w.qkv; ep.ldo = 3 * D; ep.rpb_in = rpb_in; ep.rpb_out = S; ep.row_off = row_off;
+  ep.plan = plan; ep.plan_ctx = plan_ctx;
   if (!tc_mode(e)) {
     PROF(PC_LN, launch_ln_mod(resid, D, shift, scale, ld_mod, period, a32, nullptr, nullptr, D, M, D, 1e-6f, s));
     return lin32(e, blk + "attn.qkv", a32, D, M, ep, s);
@@ -1024,21 +1042,26 @@ static int final_layer(selftok_engine* e, int B, const float* fm, float* o_out, 
 //   uncond     unconditional branch of the guided sampler (MMDiT.cfg_inference, mmdit.py:1117-1163): Kc must be 0 (no row of
 //              that pass sees a context key, so the context stream is dropped -- exact), x-stream adaLN from the integer timestep
 //   o_out      final-layer output [B*N, p*p*C]
+//   plan, Lo   token-range call: the context stream holds positions [Lo, Lo + Kc), and `plan` ([B][2] (a, c) of this step, device)
+//              tells where each image's live rows are (Epilogue / AttnPlan); NULL: the prefix [0, Kc) of every image is live
 static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_self, cudaStream_t s, bool uncond = false,
-                        float* o_out = nullptr) {
+                        float* o_out = nullptr, const int* plan = nullptr, int Lo = 0) {
   const selftok_config_t& c = e->cfg;
   DecodeWs& w = e->dws;
   const int D = e->D, N = e->Nimg, L = c.dit_depth, T = e->steps, S = Kc + N;
   const int64_t Mc = (int64_t)B * Kc, Mx = (int64_t)B * N;
   const bool ctx = Kc > 0;                                                      // is there a context stream in this pass at all
   STK_CHECK(!uncond || (!ctx && e->x_mod_u), SELFTOK_ERR_STATE, "unconditional pass needs the guided-sampler tables and no context");
+  if (!ctx) plan = nullptr;
+  AttnPlan ap;
+  ap.plan = plan; ap.n_img = N; ap.ctx_self = ctx_self;
   const float* x_mod_base = uncond ? e->x_mod_u : e->x_mod;
   for (int j = 0; j < L; ++j) {
     const bool last = j == L - 1;
     const bool ctx_post = ctx && !last;                                         // the last context block is pre_only
     const std::string pc = "model.joint_blocks." + std::to_string(j) + ".context_block.";
     const std::string px = "model.joint_blocks." + std::to_string(j) + ".x_block.";
-    const float* cmod = e->ctx_mod + (int64_t)j * c.K * 6 * D;                  // [K][6D]
+    const float* cmod = e->ctx_mod + ((int64_t)j * c.K + Lo) * 6 * D;           // [K][6D], from position Lo
     const float* xmod = x_mod_base + ((int64_t)j * T + step) * 6 * D;           // [6D]
     if (tc_mode(e)) {
       // ---- tensor-core path: the two streams' GEMMs of every stage share one launch (lintc2)
@@ -1055,11 +1078,11 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, fp16));
       TcProblem pr[2];
       Epilogue eq;                                                              // q/k/v leave the GEMM as 16-bit planes in the joint buffer
-      eq.mode = EPI_SPLIT; eq.out_hi = w.qkv_hi; eq.out_lo = w.qkv_lo; eq.ldo = 3 * D; eq.rpb_out = S;
+      eq.mode = EPI_SPLIT; eq.out_hi = w.qkv_hi; eq.out_lo = w.qkv_lo; eq.ldo = 3 * D; eq.rpb_out = S; eq.plan = plan;
       int np = 0;
-      eq.rpb_in = Kc; eq.row_off = 0;
+      eq.rpb_in = Kc; eq.row_off = 0; eq.plan_ctx = 1;
       if (ctx) STK_TRY(tc_problem(e, pc + "attn.qkv", w.a_c_hi, w.a_c_lo, Mc, eq, &pr[np++]));
-      eq.rpb_in = N; eq.row_off = Kc;
+      eq.rpb_in = N; eq.row_off = Kc; eq.plan_ctx = 0;
       STK_TRY(tc_problem(e, px + "attn.qkv", w.a_x_hi, w.a_x_lo, Mx, eq, &pr[np++]));
       STK_TRY(lintc2(e, pr, np, s));
       AttnOut ao;
@@ -1067,7 +1090,7 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       ao.hi_a = w.attn_c_hi; ao.lo_a = w.attn_c_lo; ao.hi_b = w.attn_x_hi; ao.lo_b = w.attn_x_lo;
       ao.fp16 = fp16;
       const int ctx_rows = ctx_self ? Kc : 0, ctx_keys = ctx_self ? Kc : 0;
-      PROF(PC_ATTN, launch_attention_tc5(w.qkv_hi, B, S, e->H, ctx_rows, ctx_keys, ao, s, fp16, nsplit(e) == 3 ? w.qkv_lo : nullptr));
+      PROF(PC_ATTN, launch_attention_tc5(w.qkv_hi, B, S, e->H, ctx_rows, ctx_keys, ao, s, fp16, nsplit(e) == 3 ? w.qkv_lo : nullptr, ap));
       // post_attention (mmdit.py:485-496); the pre_only context block of the last layer stops here
       Epilogue erx, erc;
       erx.mode = EPI_RESID; erx.out = w.x; erx.resid = w.x; erx.ldo = D; erx.gate = xmod + 2 * D; erx.gate_ld = 6 * D; erx.gate_period = 1;
@@ -1095,23 +1118,23 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       continue;
     }
     if (ctx && !last) {
-      STK_TRY(pre_attention(e, pc, w.ctx, Mc, cmod, cmod + D, 6 * D, Kc, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s));
+      STK_TRY(pre_attention(e, pc, w.ctx, Mc, cmod, cmod + D, 6 * D, Kc, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s, plan, 1));
     } else if (ctx) {
       const float* lm = e->ctx_last_mod + (int64_t)step * 2 * D;                // pre_only: (shift, scale) from c
-      STK_TRY(pre_attention(e, pc, w.ctx, Mc, lm, lm + D, 2 * D, 1, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s));
+      STK_TRY(pre_attention(e, pc, w.ctx, Mc, lm, lm + D, 2 * D, 1, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s, plan, 1));
     }
-    STK_TRY(pre_attention(e, px, w.x, Mx, xmod, xmod + D, 6 * D, 1, w.a_x, w.a_x_hi, w.a_x_lo, N, S, Kc, s));
+    STK_TRY(pre_attention(e, px, w.x, Mx, xmod, xmod + D, 6 * D, 1, w.a_x, w.a_x_hi, w.a_x_lo, N, S, Kc, s, plan, 0));
     AttnOut ao;
     ao.split = Kc; ao.ld = D;
     const int ctx_rows = ctx_self ? Kc : 0, ctx_keys = ctx_self ? Kc : 0;
     if (!tc_mode(e)) {
       ao.f32_a = w.attn_c; ao.f32_b = w.attn_x;
       PROF(PC_ATTN, launch_attention_f32(w.qkv, 3 * D, (int64_t)S * 3 * D, w.qkv + D, w.qkv + 2 * D, 3 * D, (int64_t)S * 3 * D, S,
-                                   nullptr, nullptr, 0, 0, 0, ao, B, S, e->H, 64, ctx_rows, ctx_keys, s));
+                                   nullptr, nullptr, 0, 0, 0, ao, B, S, e->H, 64, ctx_rows, ctx_keys, s, ap));
     } else {
       ao.hi_a = w.attn_c_hi; ao.lo_a = w.attn_c_lo; ao.hi_b = w.attn_x_hi; ao.lo_b = w.attn_x_lo;
       ao.fp16 = is_fp16(e);
-      PROF(PC_ATTN, launch_attention_tc5(w.qkv_hi, B, S, e->H, ctx_rows, ctx_keys, ao, s, is_fp16(e), nsplit(e) == 3 ? w.qkv_lo : nullptr));
+      PROF(PC_ATTN, launch_attention_tc5(w.qkv_hi, B, S, e->H, ctx_rows, ctx_keys, ao, s, is_fp16(e), nsplit(e) == 3 ? w.qkv_lo : nullptr, ap));
     }
     if (ctx_post)
       STK_TRY(post_attention(e, pc, w.ctx, Mc, cmod, 6 * D, Kc, w.attn_c, w.attn_c_hi, w.attn_c_lo, w.a_c, w.a_c_hi, w.a_c_lo,
@@ -1133,48 +1156,72 @@ static int context_embed(selftok_engine* e, int B, cudaStream_t s) {
   return lin32(e, "model.context_embedder", w.outs_q, e->cfg.code_dim, (int64_t)B * e->cfg.K, ep, s);
 }
 
+// Token-range call (selftok_*_range): per-image windows [lo_b, hi_b), rounded outward to 64 tokens for the whole batch so that one
+// captured graph serves many range sets.  Step i's context stream holds positions [Lo, Lo + Kc[i]); the per-image plan says where
+// each image's visible rows [lo_b, min(hi_b, k_i + 1)) lie in it.  Both arrays live in ws.plan (one upload per call).
+struct Window {
+  int Lo = 0, Hi = 0;
+  std::vector<int> Kc;                   // context rows per step
+  const int* range = nullptr;            // device [B][2] (lo, hi)
+  const int* plan = nullptr;             // device [steps][B][2] (a, c)
+};
+static void window_step(const Window* win, int B, int step, int k_default, int* Kc, const int** plan, int* Lo) {
+  if (!win) { *Kc = k_default; *plan = nullptr; *Lo = 0; return; }
+  *Kc = win->Kc[step];
+  *plan = *Kc > 0 ? win->plan + (int64_t)step * B * 2 : nullptr;
+  *Lo = win->Lo;
+}
+
 // One MMDiT.forward (mmdit.py:992-1101) at schedule row `step` on ws.x_lat; leaves the patch outputs in ws.o_final.
-static int dit_forward(selftok_engine* e, int B, int step, cudaStream_t s) {
+static int dit_forward(selftok_engine* e, int B, int step, cudaStream_t s, const Window* win = nullptr) {
   const selftok_config_t& c = e->cfg;
   DecodeWs& w = e->dws;
-  const int D = e->D, Kc = e->k[step] + 1;
+  const int D = e->D;
+  int Kc, Lo;
+  const int* plan;
+  window_step(win, B, step, e->k[step] + 1, &Kc, &plan, &Lo);
   PROF(PC_OTHER, launch_patchify(w.x_lat, w.patch, B, c.in_channels, c.latent, c.latent, c.dit_patch, s));
   STK_TRY(x_embed(e, B, s));
-  PROF(PC_OTHER, launch_copy_rows(w.ctx0, (int64_t)c.K * D, w.ctx, (int64_t)Kc * D, B, (int64_t)Kc * D, s));
+  if (Kc > 0) PROF(PC_OTHER, launch_copy_rows(w.ctx0 + (int64_t)Lo * D, (int64_t)c.K * D, w.ctx, (int64_t)Kc * D, B, (int64_t)Kc * D, s));
   // context rows see the image keys unless the handle was created with context_see_xt = 0 (sd3/mmdit.py:1012,1060; the
   // reference pipeline's sampler passes context_see_xt=True, SelftokPipeline.py:259)
-  return joint_blocks(e, B, Kc, step, /*ctx_self=*/e->cfg.context_see_xt == 0, s);
+  return joint_blocks(e, B, Kc, step, /*ctx_self=*/e->cfg.context_see_xt == 0, s, false, nullptr, plan, Lo);
 }
 
 // The two evaluations of one guided step (sample_one_step with cfg_scale != 1, rectified_flow.py:280-289): the conditional
 // one -- called there WITHOUT context_see_xt, i.e. context rows only see the visible context keys -- into ws.o_final, and
 // MMDiT.cfg_inference (context = zeros, every context key masked for every row: the image stream alone, integer timestep)
 // into ws.o_final_u.
-static int dit_forward_cfg(selftok_engine* e, int B, int step, cudaStream_t s) {
+static int dit_forward_cfg(selftok_engine* e, int B, int step, cudaStream_t s, const Window* win = nullptr) {
   const selftok_config_t& c = e->cfg;
   DecodeWs& w = e->dws;
-  const int D = e->D, Kc = e->k[step] + 1;
+  const int D = e->D;
+  int Kc, Lo;
+  const int* plan;
+  window_step(win, B, step, e->k[step] + 1, &Kc, &plan, &Lo);
   STK_CHECK(e->has_cfg, SELFTOK_ERR_STATE, "guided sampling needs selftok_set_cfg_schedule before selftok_finalize");
+  STK_CHECK(Kc > 0, SELFTOK_ERR_BAD_ARG, "guided sampling needs a visible context token at every step");
   PROF(PC_OTHER, launch_patchify(w.x_lat, w.patch, B, c.in_channels, c.latent, c.latent, c.dit_patch, s));
   STK_TRY(x_embed(e, B, s));
-  PROF(PC_OTHER, launch_copy_rows(w.ctx0, (int64_t)c.K * D, w.ctx, (int64_t)Kc * D, B, (int64_t)Kc * D, s));
-  STK_TRY(joint_blocks(e, B, Kc, step, /*ctx_self=*/true, s, /*uncond=*/false, w.o_final));
+  PROF(PC_OTHER, launch_copy_rows(w.ctx0 + (int64_t)Lo * D, (int64_t)c.K * D, w.ctx, (int64_t)Kc * D, B, (int64_t)Kc * D, s));
+  STK_TRY(joint_blocks(e, B, Kc, step, /*ctx_self=*/true, s, /*uncond=*/false, w.o_final, plan, Lo));
   STK_TRY(x_embed(e, B, s));
   return joint_blocks(e, B, 0, step, /*ctx_self=*/false, s, /*uncond=*/true, w.o_final_u);
 }
 
-static int decode_body(selftok_engine* e, int B, int steps, cudaStream_t s, bool guided = false, float cfg_scale = 1.f) {
+static int decode_body(selftok_engine* e, int B, int steps, cudaStream_t s, bool guided = false, float cfg_scale = 1.f,
+                       const Window* win = nullptr) {
   const selftok_config_t& c = e->cfg;
   DecodeWs& w = e->dws;
-  STK_TRY(run_lookup(e, w.tokens, B, w.outs_q, s));
+  STK_TRY(run_lookup(e, w.tokens, B, w.outs_q, s, win ? win->range : nullptr));
   STK_TRY(context_embed(e, B, s));
   for (int i = 0; i < steps; ++i) {
     // euler_step (rectified_flow.py:301-303): x <- x - (t_i - t_{i+1}) * v, fused with unpatchify
     if (!guided) {
-      STK_TRY(dit_forward(e, B, i, s));
+      STK_TRY(dit_forward(e, B, i, s, win));
       PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, w.x_lat, w.x_lat, e->dt[i], B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s));
     } else {
-      STK_TRY(dit_forward_cfg(e, B, i, s));
+      STK_TRY(dit_forward_cfg(e, B, i, s, win));
       PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, w.x_lat, w.x_lat, e->dt[i], B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s,
                                             w.o_final_u, cfg_scale));
     }
@@ -1203,8 +1250,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_set_workspace(self
   e->user_ws_bytes[op] = ws_dev ? bytes : 0;
   if (op == 0) free_ews(e);
   else {
-    for (auto& g : e->graphs) cudaGraphExecDestroy(g.second.first);
-    e->graphs.clear();
+    drop_decode_graphs(e);
     free_dws(e);
   }
   return SELFTOK_OK;
@@ -1217,7 +1263,73 @@ extern "C" __attribute__((visibility("default"))) int selftok_set_use_graph(self
 }
 
 static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const float* noise_dev, int B, int steps, float* x0_out_dev,
-                       void* stream, bool guided, float cfg_scale);
+                       void* stream, bool guided, float cfg_scale, const int32_t* range_host = nullptr);
+
+// Validates the host windows of a token-range call (before any launch) and builds its plan on the host: e->plan_host = [B][2]
+// windows then [steps][B][2] (a, c).  render: one pass, the window is not clipped by the schedule.  guided: every window must keep
+// a visible token at every executed step (the reference's conditional branch is NaN on an empty one).
+static int plan_window(selftok_engine* e, const int32_t* range_host, int B, int steps, bool render, bool guided, Window* win) {
+  STK_CHECK(range_host, SELFTOK_ERR_BAD_ARG, "token range: null range array");
+  const int K = e->cfg.K;
+  int min_k = K;
+  for (int i = 0; i < steps && !render; ++i) min_k = e->k[i] < min_k ? e->k[i] : min_k;
+  int lo_min = K, hi_max = 0;
+  for (int b = 0; b < B; ++b) {
+    const int lo = range_host[2 * b], hi = range_host[2 * b + 1];
+    if (!(0 <= lo && lo < hi && hi <= K)) {
+      set_error("token range of image " + std::to_string(b) + ": [" + std::to_string(lo) + ", " + std::to_string(hi) +
+                ") is not a window 0 <= lo < hi <= K = " + std::to_string(K));
+      return SELFTOK_ERR_BAD_ARG;
+    }
+    if (guided && lo > min_k) {
+      set_error("token range of image " + std::to_string(b) + ": the guided sampler needs lo <= k of the last step (" +
+                std::to_string(min_k) + "), got lo = " + std::to_string(lo));
+      return SELFTOK_ERR_BAD_ARG;
+    }
+    lo_min = lo < lo_min ? lo : lo_min;
+    hi_max = hi > hi_max ? hi : hi_max;
+  }
+  win->Lo = lo_min / 64 * 64;
+  win->Hi = (hi_max + 63) / 64 * 64 < K ? (hi_max + 63) / 64 * 64 : K;
+  std::vector<int>& h = e->plan_host;
+  h.assign((size_t)B * 2 * (1 + steps), 0);
+  std::copy(range_host, range_host + 2 * B, h.begin());
+  win->Kc.assign(steps, 0);
+  for (int i = 0; i < steps; ++i) {
+    const int vis_end = render ? K : e->k[i] + 1;                 // visible positions [lo_b, min(hi_b, vis_end))
+    const int end = vis_end < win->Hi ? vis_end : win->Hi;
+    win->Kc[i] = end > win->Lo ? end - win->Lo : 0;
+    for (int b = 0; b < B; ++b) {
+      const int lo = range_host[2 * b], hi = range_host[2 * b + 1];
+      const int c = (hi < vis_end ? hi : vis_end) - lo;
+      int* pr = &h[(size_t)2 * B * (1 + i) + 2 * b];
+      pr[0] = lo - win->Lo;
+      pr[1] = c > 0 ? c : 0;
+    }
+  }
+  return 0;
+}
+// uploads e->plan_host into ws.plan on the call's stream (kernels, and graphs, read it from that fixed address) through a pinned
+// staging buffer, so that the call stays asynchronous; the buffer is rewritten only after the previous upload has completed
+static int upload_window(selftok_engine* e, Window* win, int B, cudaStream_t s) {
+  DecodeWs& w = e->dws;
+  const size_t n = e->plan_host.size();
+  if (!e->plan_copied) STK_CUDA(cudaEventCreateWithFlags(&e->plan_copied, cudaEventDisableTiming));
+  else STK_CUDA(cudaEventSynchronize(e->plan_copied));
+  if (e->plan_pinned_n < n) {
+    if (e->plan_pinned) STK_CUDA(cudaFreeHost(e->plan_pinned));
+    e->plan_pinned = nullptr;
+    e->plan_pinned_n = 0;
+    STK_CUDA(cudaMallocHost(&e->plan_pinned, sizeof(int) * n));
+    e->plan_pinned_n = n;
+  }
+  memcpy(e->plan_pinned, e->plan_host.data(), sizeof(int) * n);
+  STK_CUDA(cudaMemcpyAsync(w.plan, e->plan_pinned, sizeof(int) * n, cudaMemcpyHostToDevice, s));
+  STK_CUDA(cudaEventRecord(e->plan_copied, s));
+  win->range = w.plan;
+  win->plan = w.plan + 2 * B;
+  return 0;
+}
 
 extern "C" __attribute__((visibility("default"))) int selftok_decode(selftok_handle_t e, const int64_t* tokens_dev, const float* noise_dev, int B, int steps,
                               float* x0_out_dev, void* stream) {
@@ -1231,27 +1343,54 @@ extern "C" __attribute__((visibility("default"))) int selftok_decode_cfg(selftok
   return decode_impl(e, tokens_dev, noise_dev, B, steps, x0_out_dev, stream, true, cfg_scale);
 }
 
+// Token-range entries: image b decodes from its ids [lo_b, hi_b) only (range_host: host int32 [B][2]); ids outside the window are
+// not read.  At step i the visible tokens are [lo_b, min(hi_b, k_i + 1)), the reference's `mask & super_mask`.
+extern "C" __attribute__((visibility("default"))) int selftok_decode_range(selftok_handle_t e, const int64_t* tokens_dev, const int32_t* range_host,
+                                    const float* noise_dev, int B, int steps, float* x0_out_dev, void* stream) {
+  STK_CHECK(range_host, SELFTOK_ERR_BAD_ARG, "selftok_decode_range: null range array");
+  return decode_impl(e, tokens_dev, noise_dev, B, steps, x0_out_dev, stream, false, 1.f, range_host);
+}
+extern "C" __attribute__((visibility("default"))) int selftok_decode_cfg_range(selftok_handle_t e, const int64_t* tokens_dev, const int32_t* range_host,
+                                        const float* noise_dev, int B, int steps, float cfg_scale, float* x0_out_dev,
+                                        void* stream) {
+  STK_CHECK(range_host, SELFTOK_ERR_BAD_ARG, "selftok_decode_cfg_range: null range array");
+  return decode_impl(e, tokens_dev, noise_dev, B, steps, x0_out_dev, stream, true, cfg_scale, range_host);
+}
+
 static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const float* noise_dev, int B, int steps, float* x0_out_dev,
-                       void* stream, bool guided, float cfg_scale) {
+                       void* stream, bool guided, float cfg_scale, const int32_t* range_host) {
   HOT_PROLOGUE(e);
   STK_CHECK(!guided || e->has_cfg, SELFTOK_ERR_STATE, "selftok_decode_cfg: selftok_set_cfg_schedule was not called before finalize");
   STK_CHECK(tokens_dev && noise_dev && x0_out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_decode: bad argument");
   STK_CHECK(!e->cfg.renderer, SELFTOK_ERR_STATE, "handle was created for the renderer; use selftok_render");
   STK_CHECK(steps > 0 && steps <= e->steps, SELFTOK_ERR_BAD_ARG, "steps exceeds the schedule");
+  Window win;
+  if (range_host) STK_TRY(plan_window(e, range_host, B, steps, false, guided, &win));
   STK_TRY(ensure_dws(e, B));
   DecodeWs& w = e->dws;
+  if (range_host) STK_TRY(upload_window(e, &win, B, s));
+  const Window* wp = range_host ? &win : nullptr;
   const int64_t nlat = (int64_t)B * e->cfg.in_channels * e->cfg.latent * e->cfg.latent;
   if (tokens_dev != w.tokens) STK_CUDA(cudaMemcpyAsync(w.tokens, tokens_dev, sizeof(int64_t) * B * e->cfg.K, cudaMemcpyDeviceToDevice, s));
   if (noise_dev != w.x_lat) STK_CUDA(cudaMemcpyAsync(w.x_lat, noise_dev, sizeof(float) * nlat, cudaMemcpyDeviceToDevice, s));
   // eager when asked to, for the guided loop (cfg_scale is a kernel argument) and whenever per-launch profiling is on (events
   // recorded inside a capture never execute on a real stream: their elapsed times would be garbage)
   if (!e->use_graph || guided || e->prof_on) {
-    STK_TRY(decode_body(e, B, steps, s, guided, cfg_scale));
+    STK_TRY(decode_body(e, B, steps, s, guided, cfg_scale, wp));
     e->last_launches = g_launch_count - launches0;
   } else {
-    auto key = std::make_pair(B, steps);
-    auto it = e->graphs.find(key);
-    if (it == e->graphs.end()) {
+    // token-range calls have their own graphs, keyed by the rounded window bounds: the plan itself is read at run time, so one
+    // graph serves every range set with the same (Lo, Hi)
+    const auto rkey = std::make_tuple(B, steps, win.Lo, win.Hi);
+    std::pair<cudaGraphExec_t, int64_t>* g = nullptr;
+    if (wp) {
+      auto f = e->range_graphs.find(rkey);
+      if (f != e->range_graphs.end()) g = &f->second;
+    } else {
+      auto f = e->graphs.find(std::make_pair(B, steps));
+      if (f != e->graphs.end()) g = &f->second;
+    }
+    if (!g) {
       cudaStream_t cs;
       STK_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
       {
@@ -1262,7 +1401,7 @@ static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const floa
         }
       }
       const int64_t l0 = g_launch_count;
-      int st = decode_body(e, B, steps, cs);
+      int st = decode_body(e, B, steps, cs, false, 1.f, wp);
       cudaGraph_t graph = nullptr;
       cudaError_t ce = cudaStreamEndCapture(cs, &graph);
       cudaStreamDestroy(cs);
@@ -1271,10 +1410,11 @@ static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const floa
       cudaGraphExec_t exec;
       STK_CUDA(cudaGraphInstantiate(&exec, graph, 0));
       cudaGraphDestroy(graph);
-      it = e->graphs.emplace(key, std::make_pair(exec, g_launch_count - l0)).first;
+      const auto val = std::make_pair(exec, g_launch_count - l0);
+      g = wp ? &e->range_graphs.emplace(rkey, val).first->second : &e->graphs.emplace(std::make_pair(B, steps), val).first->second;
     }
-    STK_CUDA(cudaGraphLaunch(it->second.first, s));
-    e->last_launches = it->second.second;
+    STK_CUDA(cudaGraphLaunch(g->first, s));
+    e->last_launches = g->second;
   }
   if (x0_out_dev != w.x_lat) STK_CUDA(cudaMemcpyAsync(x0_out_dev, w.x_lat, sizeof(float) * nlat, cudaMemcpyDeviceToDevice, s));
   return SELFTOK_OK;
@@ -1300,23 +1440,37 @@ extern "C" __attribute__((visibility("default"))) int selftok_dit_velocity(selft
   return SELFTOK_OK;
 }
 
-extern "C" __attribute__((visibility("default"))) int selftok_render(selftok_handle_t e, const int64_t* tokens_dev, int B, float* x0_out_dev, void* stream) {
+static int render_impl(selftok_handle_t e, const int64_t* tokens_dev, int B, float* x0_out_dev, void* stream, const int32_t* range_host) {
   HOT_PROLOGUE(e);
   STK_CHECK(tokens_dev && x0_out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_render: bad argument");
   STK_CHECK(e->cfg.renderer, SELFTOK_ERR_STATE, "handle was not created for the renderer");
+  Window win;
+  if (range_host) STK_TRY(plan_window(e, range_host, B, 1, true, false, &win));
   STK_TRY(ensure_dws(e, B));
   DecodeWs& w = e->dws;
   const selftok_config_t& c = e->cfg;
+  if (range_host) STK_TRY(upload_window(e, &win, B, s));
+  // the renderer's context: all K rows, or the rounded window [Lo, Hi) of a token-range call (no schedule clipping)
+  const int Lo = range_host ? win.Lo : 0, Kc = range_host ? win.Kc[0] : c.K;
   if (tokens_dev != w.tokens) STK_CUDA(cudaMemcpyAsync(w.tokens, tokens_dev, sizeof(int64_t) * B * c.K, cudaMemcpyDeviceToDevice, s));
-  STK_TRY(run_lookup(e, w.tokens, B, w.outs_q, s));
+  STK_TRY(run_lookup(e, w.tokens, B, w.outs_q, s, range_host ? win.range : nullptr));
   STK_TRY(context_embed(e, B, s));
-  // x = mask_token + positional_embedding (mmdit.py:1518-1522); context = full K rows, context rows see context only
+  // x = mask_token + positional_embedding (mmdit.py:1518-1522); context rows see context only
   PROF(PC_OTHER, launch_bcast_rows(e->rend_x0, nullptr, w.x, B, e->Nimg, e->D, s));
-  PROF(PC_OTHER, launch_copy_rows(w.ctx0, (int64_t)c.K * e->D, w.ctx, (int64_t)c.K * e->D, B, (int64_t)c.K * e->D, s));
-  STK_TRY(joint_blocks(e, B, c.K, 0, /*ctx_self=*/true, s));
+  PROF(PC_OTHER, launch_copy_rows(w.ctx0 + (int64_t)Lo * e->D, (int64_t)c.K * e->D, w.ctx, (int64_t)Kc * e->D, B, (int64_t)Kc * e->D, s));
+  STK_TRY(joint_blocks(e, B, Kc, 0, /*ctx_self=*/true, s, false, nullptr, range_host ? win.plan : nullptr, Lo));
   PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, nullptr, x0_out_dev, -1.f, B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s));
   e->last_launches = g_launch_count - launches0;
   return SELFTOK_OK;
+}
+extern "C" __attribute__((visibility("default"))) int selftok_render(selftok_handle_t e, const int64_t* tokens_dev, int B, float* x0_out_dev, void* stream) {
+  return render_impl(e, tokens_dev, B, x0_out_dev, stream, nullptr);
+}
+// Renderer over per-image token windows (range_host: host int32 [B][2]): MMDiT_Renderer.forward(..., mask = the window).
+extern "C" __attribute__((visibility("default"))) int selftok_render_range(selftok_handle_t e, const int64_t* tokens_dev, const int32_t* range_host, int B,
+                                    float* x0_out_dev, void* stream) {
+  STK_CHECK(range_host, SELFTOK_ERR_BAD_ARG, "selftok_render_range: null range array");
+  return render_impl(e, tokens_dev, B, x0_out_dev, stream, range_host);
 }
 
 // ------------------------------------------------------------------------------------------------ host-buffer variants
@@ -1464,5 +1618,40 @@ extern "C" __attribute__((visibility("default"))) int selftok_k_attention_tc(con
   cudaStreamSynchronize(s);
   cudaFree(qh);
   if (ql) cudaFree(ql);
+  return st;
+}
+
+// Joint attention with per-image live context counts (the token-range plan with a = 0), output in slot order [B,S,H*64].
+// live_host: host int32 [1 + B] = {Kc, c_0, ..., c_{B-1}}: every slot has Kc context rows and S - Kc image rows.
+extern "C" __attribute__((visibility("default"))) int selftok_k_attention_tc_range(const float* qkv, float* out, int B, int S, int H, int ns, int ctx_self,
+                                            const int32_t* live_host, void* stream) {
+  STK_CHECK(qkv && out && live_host && B > 0 && (ns == 0 || ns == 1 || ns == 3), SELFTOK_ERR_BAD_ARG,
+            "selftok_k_attention_tc_range: bad argument");
+  const int Kc = live_host[0];
+  STK_CHECK(Kc >= 0 && Kc < S, SELFTOK_ERR_BAD_ARG, "selftok_k_attention_tc_range: need 0 <= Kc < S");
+  std::vector<int> plan((size_t)2 * B);
+  for (int b = 0; b < B; ++b) {
+    STK_CHECK(live_host[1 + b] >= 0 && live_host[1 + b] <= Kc, SELFTOK_ERR_BAD_ARG, "selftok_k_attention_tc_range: need 0 <= c_b <= Kc");
+    plan[2 * b + 1] = live_host[1 + b];
+  }
+  const int fp16 = ns == 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t n = (int64_t)B * S * 3 * H * 64;
+  bf16 *qh, *ql = nullptr;
+  int* plan_dev;
+  STK_CUDA(cudaMalloc(&plan_dev, sizeof(int) * plan.size()));
+  STK_CUDA(cudaMemcpy(plan_dev, plan.data(), sizeof(int) * plan.size(), cudaMemcpyHostToDevice));
+  STK_CUDA(cudaMalloc(&qh, sizeof(bf16) * n));
+  if (ns == 3) STK_CUDA(cudaMalloc(&ql, sizeof(bf16) * n));
+  int st = launch_split_bf16(qkv, qh, ql, n, s, fp16);
+  AttnOut ao;
+  ao.f32_a = out; ao.split = S; ao.ld = (int64_t)H * 64;
+  AttnPlan ap;
+  ap.plan = plan_dev; ap.n_img = S - Kc; ap.ctx_self = ctx_self != 0; ap.route = 0;
+  if (!st) st = launch_attention_tc5(qh, B, S, H, 0, 0, ao, s, fp16, ql, ap);
+  cudaStreamSynchronize(s);
+  cudaFree(qh);
+  if (ql) cudaFree(ql);
+  cudaFree(plan_dev);
   return st;
 }

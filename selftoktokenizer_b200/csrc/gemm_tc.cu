@@ -59,7 +59,13 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&a
     const int64_t m = row0 + 8 * r;
     rvalid[r] = m < M;
     const int mi = (int)m;
-    orow[r] = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
+    if (e.plan && rvalid[r]) {                          // token-range plan: image rows per slot = rpb_out - Kc
+      const int b = mi / e.rpb_in;
+      const int n_img = e.rpb_out - (e.plan_ctx ? e.rpb_in : e.row_off);
+      orow[r] = b * e.rpb_out + plan_slot_row(mi % e.rpb_in, e.plan[2 * b], e.plan[2 * b + 1], n_img, e.plan_ctx != 0);
+    } else {
+      orow[r] = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
+    }
     mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
   }
 #pragma unroll

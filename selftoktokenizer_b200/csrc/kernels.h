@@ -11,6 +11,10 @@ namespace stk {
 //   mode EPI_RESID : out[orow, n] = resid[orow, n] + gate[(m % gate_period) * gate_ld + n] * y   (gate NULL -> 1)
 //   mode EPI_SPLIT : out_hi/out_lo[orow, n] = bf16 split of y            (tensor-core A-operand planes)
 // Row remap (joint attention buffer):  orow = (m / rpb_in) * rpb_out + row_off + m % rpb_in   (rpb_in == 0: orow = m)
+// Token-range plan (plan != NULL, QKV epilogues only): per image b an (a_b, c_b) pair -- its live context rows are stream rows
+// [a_b, a_b + c_b).  The image's slot of rpb_out rows then holds its live context rows, its image rows, and last its other
+// context rows (computed, never visible): plan_ctx = 1 (context stream, rpb_in = Kc): row r -> r - a_b when live, else the tail;
+// plan_ctx = 0 (image stream, rpb_in = N): row r -> c_b + r.
 enum EpiMode { EPI_STORE = 0, EPI_RESID = 1, EPI_SPLIT = 2 };
 struct Epilogue {
   int mode = EPI_STORE;
@@ -29,7 +33,14 @@ struct Epilogue {
   __nv_bfloat16* out_lo = nullptr;       // may be NULL (single-pass bf16)
   int rpb_in = 0, rpb_out = 0, row_off = 0;
   int fp16 = 0;                          // EPI_SPLIT: planes hold IEEE half (single-pass fp16 mode) instead of bf16
+  const int* plan = nullptr;             // token-range plan of this step, [B][2] int32 (a, c); NULL: plain remap
+  int plan_ctx = 0;
 };
+// slot row of stream row r of an image with plan pair (a, c); n_img = image rows per slot
+__host__ __device__ __forceinline__ int plan_slot_row(int r, int a, int c, int n_img, bool ctx) {
+  if (!ctx) return c + r;
+  return r < a ? c + n_img + r : (r < a + c ? r - a : n_img + r);
+}
 
 // ---- fp32 FFMA kernels (kernels_simt.cu) ---------------------------------------------------------------------
 int launch_linear_f32(const float* A, int64_t lda, const float* W, int64_t ldw, int64_t M, int N, int K,
@@ -63,19 +74,39 @@ struct AttnOut {
   int64_t ld = 0;
   int fp16 = 0;                          // planes hold IEEE half instead of bf16
 };
+// Token-range plan of the joint attention (plan != NULL): image b's slot of S rows holds c_b live context rows, n_img image rows,
+// then its S - c_b - n_img other context rows (see Epilogue).  Image rows see keys [0, c_b + n_img); context rows the same, or
+// [0, c_b) with ctx_self; a row with no visible key writes 0.  route != 0: output rows go back to the streams (inverse of the
+// QKV remap; AttnOut.split = Kc = S - n_img), else AttnOut's own routing applies.
+struct AttnPlan {
+  const int* plan = nullptr;             // [B][2] int32 (a, c) of this step
+  int n_img = 0;
+  int ctx_self = 0;
+  int route = 1;
+};
+// stream row of slot row `row` of an image with plan pair (a, c); ctx = whether it is a context row
+__host__ __device__ __forceinline__ int plan_stream_row(int row, int a, int c, int n_img, bool& ctx) {
+  if (row < c) { ctx = true; return a + row; }
+  if (row < c + n_img) { ctx = false; return row - c; }
+  ctx = true;
+  const int t = row - c - n_img;
+  return t < a ? t : t + c;
+}
 // softmax(q k^T / sqrt(hd)) v in fp32.  q rows: q + b*q_bs + s*q_ld + h*hd; keys = segment 1 (S1 rows) followed by
 // segment 2 (S2 rows).  Rows < ctx_rows only see keys < ctx_keys (renderer rule); ctx_rows = 0 -> dense.
 int launch_attention_f32(const float* q, int64_t q_ld, int64_t q_bs, const float* k1, const float* v1, int64_t kv1_ld,
                          int64_t kv1_bs, int S1, const float* k2, const float* v2, int64_t kv2_ld, int64_t kv2_bs,
                          int S2, const AttnOut& out, int B, int Sq, int H, int hd, int ctx_rows, int ctx_keys,
-                         cudaStream_t s);
+                         cudaStream_t s, const AttnPlan& plan = AttnPlan());
 // Fused VQ: project_in + l2norm + argmax over the codebook + gather + final_layer_norm3.
 int launch_vq(const float* z, int64_t R, int Q, const float* w_in, const float* b_in, const float* codebook,
               const float* codebook_t, int n_codes, int code_dim, const float* ln_w, const float* ln_b,
               int64_t* ids, float* outs_q, cudaStream_t s);
-// ids outside [0, n_codes): row poisoned with NaN and counted in *bad_ids (may be NULL)
+// ids outside [0, n_codes): row poisoned with NaN and counted in *bad_ids (may be NULL).  range != NULL: [R / K][2] int32 (lo, hi)
+// token windows; positions outside an image's window are not read and write a zero row.
 int launch_lookup_ln3(const int64_t* ids, int64_t R, const float* codebook, int n_codes, int code_dim,
-                      const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s);
+                      const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s,
+                      const int* range = nullptr, int K = 0);
 // [B,C,Hh,Ww] latents -> [B*(Hh/p)*(Ww/p), C*p*p] patch rows ((c,ph,pw) fastest-last, Conv2d weight order)
 int launch_patchify(const float* x, float* out, int B, int C, int Hh, int Ww, int p, cudaStream_t s);
 // x_lat[b,c,h*p+ph,w*p+pw] = x_in[...] - dt * o[b, h*g+w, (ph*p+pw)*C + c]   (unpatchify + Euler; dt = -1 & x_in NULL: plain unpatchify)
@@ -115,6 +146,6 @@ void gemm_tc_set_ctas(int n);   // 2 (default): two-CTA clusters sharing the W t
 // wgmma attention (attn_tc5.cu): single-pass 16-bit operands (fp16 != 0: IEEE half, else bf16), or -- with the lo
 // planes given -- the fp32-faithful split-bf16 mode (three MMAs per product, P split in registers)
 int launch_attention_tc5(const __nv_bfloat16* qkv16, int B, int S, int H, int ctx_rows, int ctx_keys, const AttnOut& out,
-                         cudaStream_t s, int fp16, const __nv_bfloat16* qkv_lo = nullptr);
+                         cudaStream_t s, int fp16, const __nv_bfloat16* qkv_lo = nullptr, const AttnPlan& plan = AttnPlan());
 
 }  // namespace stk

@@ -115,7 +115,13 @@ __global__ void __launch_bounds__(256, 2) linear_f32_kernel(const LinParams p) {
     const int64_t m = m0 + (i / 4) * (BM / CM) + ty * 4 + (i % 4);
     if (m >= p.M) continue;
     int64_t orow = m;
-    if (e.rpb_in > 0) orow = (m / e.rpb_in) * e.rpb_out + e.row_off + (m % e.rpb_in);
+    if (e.plan) {                                           // token-range plan: image rows per slot = rpb_out - Kc
+      const int b = (int)(m / e.rpb_in);
+      const int n_img = e.rpb_out - (e.plan_ctx ? e.rpb_in : e.row_off);
+      orow = (int64_t)b * e.rpb_out + plan_slot_row((int)(m % e.rpb_in), e.plan[2 * b], e.plan[2 * b + 1], n_img, e.plan_ctx != 0);
+    } else if (e.rpb_in > 0) {
+      orow = (m / e.rpb_in) * e.rpb_out + e.row_off + (m % e.rpb_in);
+    }
 #pragma unroll
     for (int c = 0; c < CN; ++c) {
       const int n = n0 + c * (BN / CN) + tx * 4;
@@ -461,6 +467,7 @@ struct AttnParams {
   AttnOut out;
   int Sq, H, ctx_rows, ctx_keys;
   float scale;
+  AttnPlan pl;
 };
 
 template <int HD>
@@ -489,11 +496,16 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
 #pragma unroll
     for (int d = 0; d < DV; ++d) o[i][d] = 0.f;
   }
-  // keys a row may see
+  // keys a row may see (token-range plan: this image's live context rows pc and live keys [0, live), see AttnPlan)
+  const int pc = p.pl.plan ? p.pl.plan[2 * b + 1] : 0, live = p.pl.plan ? pc + p.pl.n_img : Sk;
   int kmax_row[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) kmax_row[i] = (q0 + ty * 4 + i < p.ctx_rows) ? p.ctx_keys : Sk;
-  int kmax_cta = (q0 + BQ <= p.ctx_rows) ? p.ctx_keys : Sk;        // all rows of this CTA are context rows
+  for (int i = 0; i < 4; ++i) {
+    const int row = q0 + ty * 4 + i;
+    kmax_row[i] = !p.pl.plan ? ((row < p.ctx_rows) ? p.ctx_keys : Sk) : ((p.pl.ctx_self && (row < pc || row >= live)) ? pc : live);
+  }
+  int kmax_cta = !p.pl.plan ? ((q0 + BQ <= p.ctx_rows) ? p.ctx_keys : Sk)        // all rows of this CTA are context rows
+                            : ((p.pl.ctx_self && (q0 + BQ <= pc || q0 >= live)) ? pc : live);
   for (int k0 = 0; k0 < kmax_cta; k0 += BKV) {
     __syncthreads();                                              // previous tile fully consumed (also covers Qt)
     for (int f = tid; f < BKV * HD / 4; f += 256) {
@@ -626,10 +638,14 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
   for (int i = 0; i < 4; ++i) {
     const int row = q0 + ty * 4 + i;
     if (row >= p.Sq) continue;
-    const float inv = 1.0f / l_i[i];
+    const float inv = l_i[i] > 0.f ? 1.0f / l_i[i] : 0.f;          // a row with no visible key (token-range plan) writes 0
     const AttnOut& t = p.out;
-    const bool inA = row < t.split;
-    const int64_t orow = inA ? ((int64_t)b * t.split + row) : ((int64_t)b * (p.Sq - t.split) + (row - t.split));
+    bool inA = row < t.split;
+    int64_t orow = inA ? ((int64_t)b * t.split + row) : ((int64_t)b * (p.Sq - t.split) + (row - t.split));
+    if (p.pl.plan && p.pl.route) {
+      const int sr = plan_stream_row(row, p.pl.plan[2 * b], pc, p.pl.n_img, inA);
+      orow = inA ? (int64_t)b * t.split + sr : (int64_t)b * p.pl.n_img + sr;
+    }
     float* of = inA ? t.f32_a : t.f32_b;
     __nv_bfloat16* oh = inA ? t.hi_a : t.hi_b;
     __nv_bfloat16* ol = inA ? t.lo_a : t.lo_b;
@@ -651,12 +667,14 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
 int launch_attention_f32(const float* q, int64_t q_ld, int64_t q_bs, const float* k1, const float* v1, int64_t kv1_ld,
                          int64_t kv1_bs, int S1, const float* k2, const float* v2, int64_t kv2_ld, int64_t kv2_bs,
                          int S2, const AttnOut& out, int B, int Sq, int H, int hd, int ctx_rows, int ctx_keys,
-                         cudaStream_t s) {
+                         cudaStream_t s, const AttnPlan& plan) {
   STK_CHECK(q && k1 && v1 && B > 0 && Sq > 0 && H > 0 && S1 > 0 && S2 >= 0, -1, "attention_f32: bad arguments");
   STK_CHECK(hd == 16 || hd == 32 || hd == 64, -2, "attention_f32: head_dim must be 16, 32 or 64");
   STK_CHECK(q_ld % 4 == 0 && kv1_ld % 4 == 0 && (S2 == 0 || kv2_ld % 4 == 0), -1, "attention_f32: strides must be multiples of 4");
+  STK_CHECK(!plan.plan || (plan.n_img > 0 && plan.n_img <= Sq && (!plan.route || out.split == Sq - plan.n_img)), -1,
+            "attention_f32: inconsistent token-range plan");
   AttnParams p{q, q_ld, q_bs, k1, v1, kv1_ld, kv1_bs, S1, k2, v2, kv2_ld, kv2_bs, S2, out, Sq, H, ctx_rows, ctx_keys,
-               1.0f / sqrtf((float)hd)};
+               1.0f / sqrtf((float)hd), plan};
   dim3 grid((Sq + 63) / 64, H, B);
   size_t smem = sizeof(float) * (size_t)(hd * 68 * 2 + 64 * hd + 64 * 68);
   if (hd == 64) {
@@ -882,9 +900,16 @@ int launch_vq(const float* z, int64_t R, int Q, const float* w_in, const float* 
 // host-buffer entry points return SELFTOK_ERR_BAD_ARG).  Nothing is clamped silently.
 __global__ void lookup_ln3_kernel(const int64_t* __restrict__ ids, int64_t R, const float* __restrict__ codebook,
                                   int n_codes, int dim, const float* __restrict__ ln_w, const float* __restrict__ ln_b,
-                                  float* __restrict__ outs_q, int* __restrict__ bad_ids) {
+                                  float* __restrict__ outs_q, int* __restrict__ bad_ids, const int* __restrict__ range, int K) {
   const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= R) return;
+  if (range) {                                                  // token window: positions outside it are not read
+    const int64_t b = row / K, pos = row % K;
+    if (pos < range[2 * b] || pos >= range[2 * b + 1]) {
+      for (int d = 0; d < dim; ++d) outs_q[row * dim + d] = 0.f;
+      return;
+    }
+  }
   const int64_t id = ids[row];
   if (id < 0 || id >= n_codes) {
     if (bad_ids) atomicAdd(bad_ids, 1);
@@ -901,9 +926,11 @@ __global__ void lookup_ln3_kernel(const int64_t* __restrict__ ids, int64_t R, co
 }
 
 int launch_lookup_ln3(const int64_t* ids, int64_t R, const float* codebook, int n_codes, int code_dim,
-                      const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s) {
+                      const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s, const int* range, int K) {
   STK_CHECK(ids && codebook && ln_w && ln_b && outs_q && R > 0, -1, "lookup: bad arguments");
-  lookup_ln3_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(ids, R, codebook, n_codes, code_dim, ln_w, ln_b, outs_q, bad_ids);
+  STK_CHECK(!range || (K > 0 && R % K == 0), -1, "lookup: token windows need whole images");
+  lookup_ln3_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(ids, R, codebook, n_codes, code_dim, ln_w, ln_b, outs_q, bad_ids,
+                                                                range, K);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;

@@ -217,7 +217,8 @@ class SelftokPipeline:
         p = cfg["tokenizer"]["params"] if cfg is not None else {}
         self.cut_of_k = p.get("cut_of_k", None) or None
         if self.cut_of_k is not None:
-            raise SelftokError("cut_of_k is not on the shipped path")
+            raise SelftokError("cut_of_k is not on the shipped path (the reference's cut_of_k < 1 branch never reaches its mask hook); "
+                               "decode part of a token sequence with token_range=(lo, hi) instead")
         self.ckpt_path = ckpt_path
         self._precision_req = precision
         self._steps = 50
@@ -262,20 +263,24 @@ class SelftokPipeline:
         return self.engine.encode(x_0)
 
     @torch.no_grad()
-    def decode_latents(self, idx, noise: Optional[torch.Tensor] = None, cfg_scale: Optional[float] = None) -> torch.Tensor:
+    def decode_latents(self, idx, noise: Optional[torch.Tensor] = None, cfg_scale: Optional[float] = None, *,
+                       token_range=None) -> torch.Tensor:
         """tokens -> pred_x0 latents after the 50-step Euler loop.  `noise` defaults to the reference's draw:
         torch.randn on the CPU global generator, then moved to the device (SelftokPipeline.py:262-264).
         cfg_scale (None / 1: plain sampler): classifier-free guidance as RectifiedFlow.sample_one_step implements it
-        (rectified_flow.py:280-289) -- an explicit argument here because the reference pipeline never forwards its own."""
+        (rectified_flow.py:280-289) -- an explicit argument here because the reference pipeline never forwards its own.
+        token_range: decode image b from its ids [lo_b, hi_b) only -- a (lo, hi) pair for the batch or an int array [B, 2]; the
+        ids outside the window are not read (pad with anything).  AR models emit the sequence in reverse index order, so n
+        generated tokens = `(K - n, K)`; a truncated prefix is `(0, n)`.  Token rows stay [B, K]."""
         token_idx = torch.from_numpy(idx) if isinstance(idx, np.ndarray) else idx
         B = token_idx.shape[0]
         latent_dim = self.datasize // 8
         if noise is None:
             noise = torch.randn(B, self.dims.in_channels, latent_dim, latent_dim)
         if cfg_scale is None or float(cfg_scale) == 1.0:
-            out = self.engine.decode(token_idx, noise)
+            out = self.engine.decode(token_idx, noise, token_range=token_range)
         else:
-            out = self.engine.decode_cfg(token_idx, noise, float(cfg_scale))
+            out = self.engine.decode_cfg(token_idx, noise, float(cfg_scale), token_range=token_range)
         self._raise_on_bad_ids(token_idx)
         return out
 
@@ -286,9 +291,10 @@ class SelftokPipeline:
             raise IndexError("token id out of range for the codebook")
 
     @torch.no_grad()
-    def render_latents(self, idx) -> torch.Tensor:
+    def render_latents(self, idx, *, token_range=None) -> torch.Tensor:
+        """tokens -> pred_x0 of one renderer pass; token_range as in `decode_latents` (n generated tokens = `(K - n, K)`)."""
         token_idx = torch.from_numpy(idx) if isinstance(idx, np.ndarray) else idx
-        out = self.engine.render(token_idx)
+        out = self.engine.render(token_idx, token_range=token_range)
         self._raise_on_bad_ids(token_idx)
         return out
 
@@ -305,9 +311,10 @@ class SelftokPipeline:
 
     @torch.no_grad()
     def decode_latents_sharded(self, idx_global, noise_global: Optional[torch.Tensor] = None, seed: Optional[int] = None,
-                               gather: bool = True) -> torch.Tensor:
+                               gather: bool = True, *, token_range=None) -> torch.Tensor:
         """Global tokens [B, K] on every rank -> this rank's slice decoded; `gather` returns the global latents on every rank.
-        The initial noise is ONE host draw for the whole batch (dist.host_noise(seed)), sliced per rank."""
+        The initial noise is ONE host draw for the whole batch (dist.host_noise(seed)), sliced per rank, and so are the
+        per-image windows of `token_range` (see `decode_latents`; n generated tokens = `(K - n, K)`)."""
         from . import dist as D
         token_idx = torch.from_numpy(idx_global) if isinstance(idx_global, np.ndarray) else idx_global
         n = token_idx.shape[0]
@@ -316,7 +323,8 @@ class SelftokPipeline:
         if noise_global is None:
             latent_dim = self.datasize // 8
             noise_global = D.host_noise(n, (self.dims.in_channels, latent_dim, latent_dim), 0 if seed is None else seed)
-        out = self.engine.decode(token_idx[lo:hi], noise_global[lo:hi])
+        rng = None if token_range is None else self.engine.token_ranges(token_range, n)[lo:hi]
+        out = self.engine.decode(token_idx[lo:hi], noise_global[lo:hi], token_range=rng)
         return D.gather_rows(out, n) if gather else out
 
     # ------------------------------------------------------------------ reference API (pixel space, needs the SD3 VAE)
@@ -336,10 +344,11 @@ class SelftokPipeline:
         return tokens
 
     @torch.no_grad()
-    def decoding(self, idx, device):
+    def decoding(self, idx, device, *, token_range=None):
+        """token_range: see `decode_latents` (n generated tokens = `(K - n, K)`)."""
         print("Begin decoding.")
         self._need_vae()
-        pred_x0 = self.decode_latents(idx)
+        pred_x0 = self.decode_latents(idx, token_range=token_range)
         pred_x0_out = SD3LatentFormat().process_out(pred_x0).to(self.dtype)
         recons = self.vae.decode(pred_x0_out, return_dict=False)[0]
         norm_ip(recons, -1, 1)
@@ -347,19 +356,20 @@ class SelftokPipeline:
         return recons
 
     @torch.no_grad()
-    def decoding_cfg(self, idx, device, cfg_scale: Optional[float] = None):
-        """decoding() with the guided sampler (cfg_scale defaults to the constructor's)."""
+    def decoding_cfg(self, idx, device, cfg_scale: Optional[float] = None, *, token_range=None):
+        """decoding() with the guided sampler (cfg_scale defaults to the constructor's); token_range as in `decode_latents`."""
         self._need_vae()
-        pred_x0 = self.decode_latents(idx, cfg_scale=self.cfg_scale if cfg_scale is None else cfg_scale)
+        pred_x0 = self.decode_latents(idx, cfg_scale=self.cfg_scale if cfg_scale is None else cfg_scale, token_range=token_range)
         recons = self.vae.decode(SD3LatentFormat().process_out(pred_x0).to(self.dtype), return_dict=False)[0]
         norm_ip(recons, -1, 1)
         return recons
 
     @torch.no_grad()
-    def decoding_with_renderer(self, idx, device):
+    def decoding_with_renderer(self, idx, device, *, token_range=None):
+        """token_range: see `decode_latents` (n generated tokens = `(K - n, K)`)."""
         print("Begin decoding with Renderer.")
         self._need_vae()
-        pred_x0 = self.render_latents(idx)
+        pred_x0 = self.render_latents(idx, token_range=token_range)
         pred_x0_out = SD3LatentFormat().process_out(pred_x0).to(self.dtype)
         recons = self.vae.decode(pred_x0_out)[0]
         norm_ip(recons, -1, 1)

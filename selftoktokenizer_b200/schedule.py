@@ -111,14 +111,26 @@ def dense_flops_per_image_step(D: int, S_ctx: int, S_img: int, last_layer: bool)
     return float(f)
 
 
-def decode_flops_per_image(K: int, stages, k_per_stage, steps: int, depth: int, n_img: int) -> Tuple[float, float]:
-    """(masked-effective, dense-as-written) FLOPs of one image's `steps`-step decode (joint blocks only)."""
+def decode_flops_per_image(K: int, stages, k_per_stage, steps: int, depth: int, n_img: int,
+                           token_range: Optional[Tuple[int, int]] = None) -> Tuple[float, float]:
+    """(masked-effective, dense-as-written) FLOPs of one image's `steps`-step decode (joint blocks only).
+
+    token_range (lo, hi): (useful, executed) instead -- useful counts the image's visible tokens [lo, min(hi, k_i + 1)),
+    executed the context stream a token-range call runs, [Lo, min(Hi, k_i + 1)) with the window rounded outward to 64 tokens
+    (pass the batch's (min lo, max hi) for a mixed batch)."""
     tb = make_tables(K, stages, k_per_stage, steps)
     D = 64 * depth
+    if token_range is not None:
+        lo, hi = int(token_range[0]), int(token_range[1])
+        Lo, Hi = lo // 64 * 64, min(K, (hi + 63) // 64 * 64)
     eff = dense = 0.0
     for i in range(steps):
         kc = int(tb.k[i]) + 1
+        if token_range is None:
+            rows_a, rows_b = kc, K
+        else:
+            rows_a, rows_b = max(0, min(hi, kc) - lo), max(0, min(Hi, kc) - Lo)
         for layer in range(depth):
-            eff += dense_flops_per_image_step(D, kc, n_img, layer == depth - 1)
-            dense += dense_flops_per_image_step(D, K, n_img, layer == depth - 1)
+            eff += dense_flops_per_image_step(D, rows_a, n_img, layer == depth - 1)
+            dense += dense_flops_per_image_step(D, rows_b, n_img, layer == depth - 1)
     return eff, dense
