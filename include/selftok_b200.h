@@ -165,6 +165,26 @@ int selftok_decode_cfg_range(selftok_handle_t h, const int64_t* tokens_dev, cons
 int selftok_render_range(selftok_handle_t h, const int64_t* tokens_dev, const int32_t* range_host, int B, float* x0_out_dev,
                          void* stream);
 
+/* ---- step-level batching (continuous batching of the sampler) ------------------------------------------------
+ * One Euler step per image, each at its own schedule row s_b = step_host[b] (host int32 [B]):
+ *   x_out[b] = x[b] - dt[s_b] * v_b        (sd3/rectified_flow.py:301-303)
+ * cfg_scale_host == NULL: v_b is selftok_decode's velocity at row s_b; else (host float [B]) the guided combination
+ * v_u + cfg_scale_host[b] * (v_c - v_u) of one selftok_decode_cfg step.  A call is all plain or all guided.
+ * tokens_dev [B,K] int64, x_dev / x_out_dev [B,C,latent,latent] fp32 (x_out_dev may alias x_dev); range_host: host int32 [B][2]
+ * windows as for selftok_decode_range, NULL = [0, K) for every image.  Image b sees the ids [lo_b, min(hi_b, k_{s_b} + 1));
+ * ids outside them are not read, validated or counted by selftok_id_errors.
+ * Before any launch (selftok_last_error() names the image): a step outside [0, steps), a bad window, or -- guided -- an image
+ * without a visible token at its step is SELFTOK_ERR_BAD_ARG, as are NULL pointers and B <= 0; a renderer handle, or a guided
+ * call on a handle without selftok_set_cfg_schedule, is SELFTOK_ERR_STATE.
+ * Contract: running steps 0..n-1 of an image through any sequence of calls -- in any batches, interleaved in any order with
+ * other images -- gives bitwise what selftok_decode(steps = n) (selftok_decode_range with its window; selftok_decode_cfg(_range)
+ * with its scale) gives for that image.  The entry is stateless (the caller owns tokens, latents and step indices) and
+ * asynchronous: its per-image block goes up through the handle's pinned staging buffer.  It runs eager (selftok_set_use_graph
+ * does not apply) in the decode workspace.  The context stream is packed: image b contributes exactly its visible rows, so the
+ * executed work is the useful work whatever mix of steps a batch holds. */
+int selftok_decode_step(selftok_handle_t h, const int64_t* tokens_dev, const int32_t* range_host, const int32_t* step_host,
+                        const float* cfg_scale_host, const float* x_dev, int B, float* x_out_dev, void* stream);
+
 /* ---- hot path, host buffers (what SelftokPipeline's numpy-in / tensor-out API maps to; H2D and D2H copies are
  * inside the call, on `stream`, followed by a stream synchronize) --------------------------------------------- */
 int selftok_encode_host(selftok_handle_t h, const float* x0_host, int B, int64_t* tokens_host, void* stream);

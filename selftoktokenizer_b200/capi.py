@@ -27,6 +27,7 @@ SYMBOLS = [
     "selftok_render_host", "selftok_id_errors", "selftok_workspace_bytes", "selftok_set_workspace", "selftok_last_launch_count", "selftok_device_bytes", "selftok_set_use_graph",
     "selftok_set_profile", "selftok_get_profile", "selftok_k_linear_f32", "selftok_k_linear_tc", "selftok_k_set_gemm_ctas", "selftok_k_ln_mod_f32", "selftok_k_attention_f32",
     "selftok_k_attention_tc", "selftok_decode_range", "selftok_decode_cfg_range", "selftok_render_range", "selftok_k_attention_tc_range",
+    "selftok_decode_step",
     "selftok_vae_create", "selftok_vae_destroy", "selftok_vae_load_tensor", "selftok_vae_finalize", "selftok_vae_decode", "selftok_vae_encode", "selftok_vae_device_bytes",
 ]
 
@@ -98,6 +99,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.selftok_decode_cfg_range.argtypes = [vp, vp, vp, vp, i32, i32, C.c_float, vp, vp]
     lib.selftok_render_range.argtypes = [vp, vp, vp, i32, vp, vp]
     lib.selftok_k_attention_tc_range.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp]
+    lib.selftok_decode_step.argtypes = [vp, vp, vp, vp, vp, vp, i32, vp, vp]
     lib.selftok_vae_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.selftok_vae_destroy.argtypes = [vp]
     lib.selftok_vae_load_tensor.argtypes = [vp, C.c_char_p, vp, i32, C.POINTER(i64), i32]
@@ -374,6 +376,49 @@ class Engine:
             else:
                 check(self.lib.selftok_decode_cfg_range(self.h, tokens.data_ptr(), rng.ctypes.data, noise.data_ptr(), tokens.shape[0],
                                                         steps or self.steps, float(cfg_scale), out.data_ptr(), _stream_ptr(self.device)))
+        return out
+
+    def decode_step(self, tokens: torch.Tensor, x: torch.Tensor, step, *, token_range=None, cfg_scale=None,
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """One Euler step per image at its own schedule row (selftok_decode_step): x [B,C,h,w] -> x - dt[step_b] * v_b.
+        `step`: an int for the whole batch or an int array [B].  cfg_scale: None (plain sampler), a float or a float array [B]
+        (guided sampler, every image).  token_range as in `decode`.  `out` may be `x` itself.  Running steps 0..n-1 of an image
+        through any sequence of calls, in any batches, is bitwise `decode(steps=n)` / `decode_cfg` of that image alone."""
+        self._check_latent(x, "decode_step (x)")
+        B = x.shape[0]
+        rng = None if token_range is None else self.token_ranges(token_range, B)
+        st = np.asarray(step)
+        if st.shape == ():
+            st = np.broadcast_to(st, (B,))
+        if st.shape != (B,) or not np.issubdtype(st.dtype, np.integer):
+            raise SelftokError(f"decode_step: step must be an int or an int array [{B}], got {st.dtype} {st.shape}")
+        st = np.ascontiguousarray(st, dtype=np.int32)
+        cs = None
+        if cfg_scale is not None:
+            cs = np.asarray(cfg_scale, dtype=np.float32)
+            if cs.shape == ():
+                cs = np.broadcast_to(cs, (B,))
+            if cs.shape != (B,):
+                raise SelftokError(f"decode_step: cfg_scale must be a float or a float array [{B}], got shape {cs.shape}")
+            cs = np.ascontiguousarray(cs, dtype=np.float32)
+        if tokens.dim() != 2 or tokens.shape[1] != self.dims.K or tokens.shape[0] != B:
+            raise SelftokError(f"decode_step: expected [{B}, {self.dims.K}] token ids, got {tuple(tokens.shape)}")
+        if not tokens.is_cuda:
+            # only the ids visible at each image's step are read: check exactly those
+            lo = np.zeros(B, np.int64) if rng is None else rng[:, 0].astype(np.int64)
+            hi = np.full(B, self.dims.K, np.int64) if rng is None else rng[:, 1].astype(np.int64)
+            k = self.tables.k.numpy().astype(np.int64)[np.clip(st, 0, self.steps - 1)]
+            self._check_tokens(tokens, "decode_step", B, ranges=np.stack([lo, np.minimum(hi, k + 1)], 1).astype(np.int32))
+        tokens = self._dev(tokens, torch.int64)
+        x = self._dev(x, torch.float32)
+        if out is None:
+            out = torch.empty_like(x)
+        elif out.shape != x.shape or out.dtype != torch.float32 or out.device != x.device or not out.is_contiguous():
+            raise SelftokError("decode_step: `out` must be a contiguous fp32 device tensor shaped like x")
+        with torch.cuda.device(self.device):
+            check(self.lib.selftok_decode_step(self.h, tokens.data_ptr(), None if rng is None else rng.ctypes.data, st.ctypes.data,
+                                               None if cs is None else cs.ctypes.data, x.data_ptr(), B, out.data_ptr(),
+                                               _stream_ptr(self.device)))
         return out
 
     def dit_velocity(self, tokens: torch.Tensor, x: torch.Tensor, step: int) -> torch.Tensor:

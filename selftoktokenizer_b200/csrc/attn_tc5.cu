@@ -106,6 +106,7 @@ attention_tc5_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                                   : ((p.pl.ctx_self && ((qt + 1) * BQ <= pc || qt * BQ >= live)) ? pc : live);
   const int n_tiles = (kmax_cta + BKV - 1) / BKV;
   const int row0 = b * S;                                     // first row of this image in the [B*S, 3*H*64] matrix
+  if (p.pl.packed && qt * BQ >= live) return;                 // packed slot: no row of this tile holds anything
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&map_q);
@@ -236,7 +237,11 @@ attention_tc5_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     const float inv = l > 0.f ? 1.0f / l : 0.f;                // a row with no visible key (token-range plan) writes 0
     bool inA = row < t.split;
     int64_t orow = inA ? ((int64_t)b * t.split + row) : ((int64_t)b * (S - t.split) + (row - t.split));
-    if (p.pl.plan && p.pl.route) {
+    if (p.pl.packed) {
+      if (row >= live) continue;
+      inA = row < pc;
+      orow = inA ? (int64_t)p.pl.plan[2 * b] + row : (int64_t)b * p.pl.n_img + row - pc;
+    } else if (p.pl.plan && p.pl.route) {
       const int sr = plan_stream_row(row, p.pl.plan[2 * b], pc, p.pl.n_img, inA);
       orow = inA ? (int64_t)b * t.split + sr : (int64_t)b * p.pl.n_img + sr;
     }

@@ -70,6 +70,7 @@ struct DecodeWs {       // activation workspace of the MMDiT for one batch size
   bf16 *attn_c_hi = nullptr, *attn_c_lo = nullptr, *attn_x_hi = nullptr, *attn_x_lo = nullptr;
   bf16 *h_c_hi = nullptr, *h_c_lo = nullptr, *h_x_hi = nullptr, *h_x_lo = nullptr;
   int* plan = nullptr;                           // token-range calls: [B][2] windows (lo, hi), then the plan [steps][B][2] (a, c)
+  int* pk = nullptr;                             // step calls: the per-image block (see Packed), then the per-row maps
   void* own = nullptr;                           // the library's own block (NULL when the caller's workspace is in use)
   size_t own_bytes = 0;
 };
@@ -851,12 +852,14 @@ extern "C" __attribute__((visibility("default"))) int selftok_vq_argmax(selftok_
 }
 
 // range != NULL: device [B][2] token windows; ids outside an image's window are not read (zero rows)
-static int run_lookup(selftok_engine* e, const int64_t* tokens, int B, float* outs_q, cudaStream_t s, const int* range = nullptr) {
+// gather != NULL: R rows of a packed context stream, row m from tokens[gather[m]]
+static int run_lookup(selftok_engine* e, const int64_t* tokens, int B, float* outs_q, cudaStream_t s, const int* range = nullptr,
+                      const int* gather = nullptr, int64_t R = 0) {
   GETW(cb, "encoder.quantizer._codebook.embed");
   GETW(lw, "encoder.final_layer_norm3.weight");
   GETW(lb, "encoder.final_layer_norm3.bias");
-  PROF(PC_OTHER, launch_lookup_ln3(tokens, (int64_t)B * e->cfg.K, cb->d, e->cfg.codebook_size, e->cfg.code_dim, lw->d, lb->d, outs_q,
-                                   e->bad_ids, s, range, e->cfg.K));
+  PROF(PC_OTHER, launch_lookup_ln3(tokens, gather ? R : (int64_t)B * e->cfg.K, cb->d, e->cfg.codebook_size, e->cfg.code_dim, lw->d, lb->d,
+                                   outs_q, e->bad_ids, s, range, e->cfg.K, gather));
   return 0;
 }
 
@@ -891,6 +894,19 @@ extern "C" __attribute__((visibility("default"))) int selftok_lookup(selftok_han
 }
 
 // ------------------------------------------------------------------------------------------------ decode
+// A step call (selftok_decode_step) runs one Euler step for images at their own schedule rows over a PACKED context stream: image
+// b contributes exactly its c_b visible rows, at stream rows [off_b, off_b + c_b).  Its joint-attention slot of S = max c + N rows
+// holds those c_b rows, then its N image rows.  Per-image block uploaded once per call (ws.pk, int32):
+//   [B][2] (off_b, c_b) | [B] lo_b | [B] step_b | [B] dt of step_b (float) | [B] cfg scale (float)
+// followed by the per-row maps launch_expand_packed derives from it on the device.
+constexpr int PK_IMG_INTS = 6;
+struct Packed {
+  int Mc = 0, S = 0;                                   // context stream rows (sum of c_b), joint slot rows
+  const int* pair = nullptr;                           // [B][2] (off_b, c_b)
+  const float *dt = nullptr, *scale = nullptr;         // [B]
+  const int *ctx_tok = nullptr, *ctx_pos = nullptr, *ctx_step = nullptr, *ctx_dst = nullptr;   // [Mc]
+  const int* x_step = nullptr;                         // [B N]
+};
 static int layout_dws(selftok_engine* e, DecodeWs& w, int64_t B, Arena& A) {
   const selftok_config_t& c = e->cfg;
   const int64_t K = c.K, N = e->Nimg, D = e->D, S = K + N;
@@ -905,6 +921,7 @@ static int layout_dws(selftok_engine* e, DecodeWs& w, int64_t B, Arena& A) {
   STK_TRY(A.take(&w.o_final_u, B * N * c.dit_patch * c.dit_patch * c.in_channels));
   STK_TRY(A.take(&w.a_x, B * N * D));                       // fp32 LN output of the final layer (both modes)
   STK_TRY(A.take(&w.plan, B * 2 * (1 + (int64_t)e->steps)));
+  STK_TRY(A.take(&w.pk, B * (PK_IMG_INTS + 4 * K + N)));
   if (!tc_mode(e)) {
     STK_TRY(A.take(&w.qkv, B * S * 3 * D));
     STK_TRY(A.take(&w.a_c, B * K * D));
@@ -953,17 +970,18 @@ static int ensure_dws(selftok_engine* e, int B) {
 // One stream of one JointBlock: LN+modulate -> qkv GEMM into the joint buffer   (mmdit.py:441-483, 521-529)
 static int pre_attention(selftok_engine* e, const std::string& blk, const float* resid, int64_t M, const float* shift,
                          const float* scale, int64_t ld_mod, int period, float* a32, bf16* a_hi, bf16* a_lo, int rpb_in,
-                         int S, int row_off, cudaStream_t s, const int* plan = nullptr, int plan_ctx = 0) {
+                         int S, int row_off, cudaStream_t s, const int* plan = nullptr, int plan_ctx = 0, const int* rows = nullptr,
+                         const int* row_map = nullptr) {
   const int D = e->D;
   DecodeWs& w = e->dws;
   Epilogue ep;
   ep.out = w.qkv; ep.ldo = 3 * D; ep.rpb_in = rpb_in; ep.rpb_out = S; ep.row_off = row_off;
-  ep.plan = plan; ep.plan_ctx = plan_ctx;
+  ep.plan = plan; ep.plan_ctx = plan_ctx; ep.row_map = row_map;
   if (!tc_mode(e)) {
-    PROF(PC_LN, launch_ln_mod(resid, D, shift, scale, ld_mod, period, a32, nullptr, nullptr, D, M, D, 1e-6f, s));
+    PROF(PC_LN, launch_ln_mod(resid, D, shift, scale, ld_mod, period, a32, nullptr, nullptr, D, M, D, 1e-6f, s, 0, rows));
     return lin32(e, blk + "attn.qkv", a32, D, M, ep, s);
   }
-  PROF(PC_LN, launch_ln_mod(resid, D, shift, scale, ld_mod, period, nullptr, a_hi, a_lo, D, M, D, 1e-6f, s, is_fp16(e)));
+  PROF(PC_LN, launch_ln_mod(resid, D, shift, scale, ld_mod, period, nullptr, a_hi, a_lo, D, M, D, 1e-6f, s, is_fp16(e), rows));
   ep.mode = EPI_SPLIT; ep.out = nullptr; ep.out_hi = w.qkv_hi; ep.out_lo = w.qkv_lo;      // q/k/v leave the GEMM as 16-bit planes
   return lintc(e, blk + "attn.qkv", a_hi, a_lo, M, ep, s);
 }
@@ -971,23 +989,23 @@ static int pre_attention(selftok_engine* e, const std::string& blk, const float*
 // post_attention (mmdit.py:485-496): x += gate_msa*proj(attn); x += gate_mlp*mlp(modulate(norm2(x)))
 static int post_attention(selftok_engine* e, const std::string& blk, float* resid, int64_t M, const float* mod, int64_t ld_mod,
                           int period, const float* attn32, const bf16* attn_hi, const bf16* attn_lo, float* a32, bf16* a_hi,
-                          bf16* a_lo, float* h32, bf16* h_hi, bf16* h_lo, cudaStream_t s) {
+                          bf16* a_lo, float* h32, bf16* h_hi, bf16* h_lo, cudaStream_t s, const int* rows = nullptr) {
   const int D = e->D;
   Epilogue er;
   er.mode = EPI_RESID; er.out = resid; er.resid = resid; er.ldo = D;
-  er.gate = mod + 2 * D; er.gate_ld = ld_mod; er.gate_period = period;
+  er.gate = mod + 2 * D; er.gate_ld = ld_mod; er.gate_period = period; er.tab_rows = rows;
   Epilogue eh;
   eh.act = ACT_GELU;
   if (!tc_mode(e)) {
     STK_TRY(lin32(e, blk + "attn.proj", attn32, D, M, er, s));
-    PROF(PC_LN, launch_ln_mod(resid, D, mod + 3 * D, mod + 4 * D, ld_mod, period, a32, nullptr, nullptr, D, M, D, 1e-6f, s));
+    PROF(PC_LN, launch_ln_mod(resid, D, mod + 3 * D, mod + 4 * D, ld_mod, period, a32, nullptr, nullptr, D, M, D, 1e-6f, s, 0, rows));
     eh.out = h32; eh.ldo = 4 * D;
     STK_TRY(lin32(e, blk + "mlp.fc1", a32, D, M, eh, s));
     er.gate = mod + 5 * D;
     return lin32(e, blk + "mlp.fc2", h32, 4 * D, M, er, s);
   }
   STK_TRY(lintc(e, blk + "attn.proj", attn_hi, attn_lo, M, er, s));
-  PROF(PC_LN, launch_ln_mod(resid, D, mod + 3 * D, mod + 4 * D, ld_mod, period, nullptr, a_hi, a_lo, D, M, D, 1e-6f, s, is_fp16(e)));
+  PROF(PC_LN, launch_ln_mod(resid, D, mod + 3 * D, mod + 4 * D, ld_mod, period, nullptr, a_hi, a_lo, D, M, D, 1e-6f, s, is_fp16(e), rows));
   eh.mode = EPI_SPLIT; eh.out_hi = h_hi; eh.out_lo = h_lo; eh.ldo = 4 * D;
   STK_TRY(lintc(e, blk + "mlp.fc1", a_hi, a_lo, M, eh, s));
   er.gate = mod + 5 * D;
@@ -1012,18 +1030,20 @@ static int x_embed(selftok_engine* e, int B, cudaStream_t s) {
   return 0;
 }
 // FinalLayer (mmdit.py:641-645): LN + modulate, then the N = p*p*C = 64 column linear -> o_out [B*N, 64] fp32
-static int final_layer(selftok_engine* e, int B, const float* fm, float* o_out, cudaStream_t s) {
+// rows != NULL: per-row rows of the fm table (packed step calls), else its single row
+static int final_layer(selftok_engine* e, int B, const float* fm, float* o_out, cudaStream_t s, const int* rows = nullptr) {
   DecodeWs& w = e->dws;
   const int D = e->D;
   const int64_t Mx = (int64_t)B * e->Nimg;
   if (!tc_mode(e)) {
-    PROF(PC_LN, launch_ln_mod(w.x, D, fm, fm + D, 2 * D, 1, w.a_x, nullptr, nullptr, D, Mx, D, 1e-6f, s));
+    PROF(PC_LN, launch_ln_mod(w.x, D, fm, fm + D, 2 * D, 1, w.a_x, nullptr, nullptr, D, Mx, D, 1e-6f, s, 0, rows));
     Epilogue ep;
     ep.out = o_out;
     return lin32(e, "model.final_layer.linear", w.a_x, D, Mx, ep, s);
   }
   LnProblem lp;
   lp.x = w.x; lp.shift = fm; lp.scale = fm + D; lp.ld_mod = 2 * D; lp.period = 1; lp.out_hi = w.fin_hi; lp.out_lo = w.fin_lo; lp.M = Mx;
+  lp.rows = rows;
   PROF(PC_LN, launch_ln_mod_pair(&lp, 1, D, 1e-6f, s, 0));
   GETW(W, "model.final_layer.linear.weight");
   GETW(Bv, "model.final_layer.linear.bias");
@@ -1044,18 +1064,26 @@ static int final_layer(selftok_engine* e, int B, const float* fm, float* o_out, 
 //   o_out      final-layer output [B*N, p*p*C]
 //   plan, Lo   token-range call: the context stream holds positions [Lo, Lo + Kc), and `plan` ([B][2] (a, c) of this step, device)
 //              tells where each image's live rows are (Epilogue / AttnPlan); NULL: the prefix [0, Kc) of every image is live
+//   pk         step call (Kc, step, plan and Lo unused): packed context stream of pk->Mc rows (Mc = 0: none), every table row
+//              taken from the per-row maps
 static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_self, cudaStream_t s, bool uncond = false,
-                        float* o_out = nullptr, const int* plan = nullptr, int Lo = 0) {
+                        float* o_out = nullptr, const int* plan = nullptr, int Lo = 0, const Packed* pk = nullptr) {
   const selftok_config_t& c = e->cfg;
   DecodeWs& w = e->dws;
+  if (pk) { step = 0; Lo = 0; plan = pk->pair; Kc = pk->S - e->Nimg; }
   const int D = e->D, N = e->Nimg, L = c.dit_depth, T = e->steps, S = Kc + N;
-  const int64_t Mc = (int64_t)B * Kc, Mx = (int64_t)B * N;
-  const bool ctx = Kc > 0;                                                      // is there a context stream in this pass at all
+  const int64_t Mc = pk ? pk->Mc : (int64_t)B * Kc, Mx = (int64_t)B * N;
+  const bool ctx = Mc > 0;                                                      // is there a context stream in this pass at all
   STK_CHECK(!uncond || (!ctx && e->x_mod_u), SELFTOK_ERR_STATE, "unconditional pass needs the guided-sampler tables and no context");
   if (!ctx) plan = nullptr;
   AttnPlan ap;
-  ap.plan = plan; ap.n_img = N; ap.ctx_self = ctx_self;
+  ap.plan = plan; ap.n_img = N; ap.ctx_self = ctx_self; ap.packed = pk && ctx;
   const float* x_mod_base = uncond ? e->x_mod_u : e->x_mod;
+  // per-row table rows of a step call: context rows by position (last layer: by step), image rows by step
+  const int* rows_c = pk ? pk->ctx_pos : nullptr;
+  const int* rows_cl = pk ? pk->ctx_step : nullptr;
+  const int* rows_x = pk ? pk->x_step : nullptr;
+  const int* map_c = pk ? pk->ctx_dst : nullptr;
   for (int j = 0; j < L; ++j) {
     const bool last = j == L - 1;
     const bool ctx_post = ctx && !last;                                         // the last context block is pre_only
@@ -1070,19 +1098,19 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       // LN + modulate of both streams in one launch (context rows: per-position adaLN table; image rows: the step's row)
       LnProblem lp[2];
       lp[0].x = w.ctx; lp[0].out_hi = w.a_c_hi; lp[0].out_lo = w.a_c_lo; lp[0].M = Mc;
-      if (!last) { lp[0].shift = cmod; lp[0].scale = cmod + D; lp[0].ld_mod = 6 * D; lp[0].period = Kc; }
-      else { lp[0].shift = lm; lp[0].scale = lm + D; lp[0].ld_mod = 2 * D; lp[0].period = 1; }
+      if (!last) { lp[0].shift = cmod; lp[0].scale = cmod + D; lp[0].ld_mod = 6 * D; lp[0].period = Kc; lp[0].rows = rows_c; }
+      else { lp[0].shift = lm; lp[0].scale = lm + D; lp[0].ld_mod = 2 * D; lp[0].period = 1; lp[0].rows = rows_cl; }
       lp[1].x = w.x; lp[1].out_hi = w.a_x_hi; lp[1].out_lo = w.a_x_lo; lp[1].M = Mx;
-      lp[1].shift = xmod; lp[1].scale = xmod + D; lp[1].ld_mod = 6 * D; lp[1].period = 1;
+      lp[1].shift = xmod; lp[1].scale = xmod + D; lp[1].ld_mod = 6 * D; lp[1].period = 1; lp[1].rows = rows_x;
       if (ctx) PROF(PC_LN, launch_ln_mod_pair(lp, 2, D, 1e-6f, s, fp16));
       else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, fp16));
       TcProblem pr[2];
       Epilogue eq;                                                              // q/k/v leave the GEMM as 16-bit planes in the joint buffer
       eq.mode = EPI_SPLIT; eq.out_hi = w.qkv_hi; eq.out_lo = w.qkv_lo; eq.ldo = 3 * D; eq.rpb_out = S; eq.plan = plan;
       int np = 0;
-      eq.rpb_in = Kc; eq.row_off = 0; eq.plan_ctx = 1;
+      eq.rpb_in = Kc; eq.row_off = 0; eq.plan_ctx = 1; eq.row_map = map_c;
       if (ctx) STK_TRY(tc_problem(e, pc + "attn.qkv", w.a_c_hi, w.a_c_lo, Mc, eq, &pr[np++]));
-      eq.rpb_in = N; eq.row_off = Kc; eq.plan_ctx = 0;
+      eq.rpb_in = N; eq.row_off = Kc; eq.plan_ctx = 0; eq.row_map = nullptr;
       STK_TRY(tc_problem(e, px + "attn.qkv", w.a_x_hi, w.a_x_lo, Mx, eq, &pr[np++]));
       STK_TRY(lintc2(e, pr, np, s));
       AttnOut ao;
@@ -1095,11 +1123,12 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       Epilogue erx, erc;
       erx.mode = EPI_RESID; erx.out = w.x; erx.resid = w.x; erx.ldo = D; erx.gate = xmod + 2 * D; erx.gate_ld = 6 * D; erx.gate_period = 1;
       erc.mode = EPI_RESID; erc.out = w.ctx; erc.resid = w.ctx; erc.ldo = D; erc.gate = cmod + 2 * D; erc.gate_ld = 6 * D; erc.gate_period = Kc;
+      erx.tab_rows = rows_x; erc.tab_rows = rows_c;
       np = 0;
       if (ctx_post) STK_TRY(tc_problem(e, pc + "attn.proj", w.attn_c_hi, w.attn_c_lo, Mc, erc, &pr[np++]));
       STK_TRY(tc_problem(e, px + "attn.proj", w.attn_x_hi, w.attn_x_lo, Mx, erx, &pr[np++]));
       STK_TRY(lintc2(e, pr, np, s));
-      lp[0].shift = cmod + 3 * D; lp[0].scale = cmod + 4 * D; lp[0].ld_mod = 6 * D; lp[0].period = Kc;
+      lp[0].shift = cmod + 3 * D; lp[0].scale = cmod + 4 * D; lp[0].ld_mod = 6 * D; lp[0].period = Kc; lp[0].rows = rows_c;
       lp[1].shift = xmod + 3 * D; lp[1].scale = xmod + 4 * D;
       if (ctx_post) PROF(PC_LN, launch_ln_mod_pair(lp, 2, D, 1e-6f, s, fp16));
       else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, fp16));
@@ -1118,12 +1147,12 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       continue;
     }
     if (ctx && !last) {
-      STK_TRY(pre_attention(e, pc, w.ctx, Mc, cmod, cmod + D, 6 * D, Kc, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s, plan, 1));
+      STK_TRY(pre_attention(e, pc, w.ctx, Mc, cmod, cmod + D, 6 * D, Kc, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s, plan, 1, rows_c, map_c));
     } else if (ctx) {
       const float* lm = e->ctx_last_mod + (int64_t)step * 2 * D;                // pre_only: (shift, scale) from c
-      STK_TRY(pre_attention(e, pc, w.ctx, Mc, lm, lm + D, 2 * D, 1, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s, plan, 1));
+      STK_TRY(pre_attention(e, pc, w.ctx, Mc, lm, lm + D, 2 * D, 1, w.a_c, w.a_c_hi, w.a_c_lo, Kc, S, 0, s, plan, 1, rows_cl, map_c));
     }
-    STK_TRY(pre_attention(e, px, w.x, Mx, xmod, xmod + D, 6 * D, 1, w.a_x, w.a_x_hi, w.a_x_lo, N, S, Kc, s, plan, 0));
+    STK_TRY(pre_attention(e, px, w.x, Mx, xmod, xmod + D, 6 * D, 1, w.a_x, w.a_x_hi, w.a_x_lo, N, S, Kc, s, plan, 0, rows_x));
     AttnOut ao;
     ao.split = Kc; ao.ld = D;
     const int ctx_rows = ctx_self ? Kc : 0, ctx_keys = ctx_self ? Kc : 0;
@@ -1138,12 +1167,12 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
     }
     if (ctx_post)
       STK_TRY(post_attention(e, pc, w.ctx, Mc, cmod, 6 * D, Kc, w.attn_c, w.attn_c_hi, w.attn_c_lo, w.a_c, w.a_c_hi, w.a_c_lo,
-                             w.h_c, w.h_c_hi, w.h_c_lo, s));
+                             w.h_c, w.h_c_hi, w.h_c_lo, s, rows_c));
     STK_TRY(post_attention(e, px, w.x, Mx, xmod, 6 * D, 1, w.attn_x, w.attn_x_hi, w.attn_x_lo, w.a_x, w.a_x_hi, w.a_x_lo,
-                           w.h_x, w.h_x_hi, w.h_x_lo, s));
+                           w.h_x, w.h_x_hi, w.h_x_lo, s, rows_x));
   }
   const float* fm = (uncond ? e->final_mod_u : e->final_mod) + (int64_t)step * 2 * D;
-  return final_layer(e, B, fm, o_out ? o_out : w.o_final, s);
+  return final_layer(e, B, fm, o_out ? o_out : w.o_final, s, rows_x);
 }
 
 // context_embedder(outs_q) + context_pos_embed (mmdit.py:1026) — step invariant, computed once per call
@@ -1309,10 +1338,9 @@ static int plan_window(selftok_engine* e, const int32_t* range_host, int B, int 
   }
   return 0;
 }
-// uploads e->plan_host into ws.plan on the call's stream (kernels, and graphs, read it from that fixed address) through a pinned
-// staging buffer, so that the call stays asynchronous; the buffer is rewritten only after the previous upload has completed
-static int upload_window(selftok_engine* e, Window* win, int B, cudaStream_t s) {
-  DecodeWs& w = e->dws;
+// uploads e->plan_host to dst on the call's stream (kernels, and graphs, read it from that fixed address) through a pinned staging
+// buffer, so that the call stays asynchronous; the buffer is rewritten only after the previous upload has completed
+static int upload_plan(selftok_engine* e, int* dst, cudaStream_t s) {
   const size_t n = e->plan_host.size();
   if (!e->plan_copied) STK_CUDA(cudaEventCreateWithFlags(&e->plan_copied, cudaEventDisableTiming));
   else STK_CUDA(cudaEventSynchronize(e->plan_copied));
@@ -1324,8 +1352,13 @@ static int upload_window(selftok_engine* e, Window* win, int B, cudaStream_t s) 
     e->plan_pinned_n = n;
   }
   memcpy(e->plan_pinned, e->plan_host.data(), sizeof(int) * n);
-  STK_CUDA(cudaMemcpyAsync(w.plan, e->plan_pinned, sizeof(int) * n, cudaMemcpyHostToDevice, s));
+  STK_CUDA(cudaMemcpyAsync(dst, e->plan_pinned, sizeof(int) * n, cudaMemcpyHostToDevice, s));
   STK_CUDA(cudaEventRecord(e->plan_copied, s));
+  return 0;
+}
+static int upload_window(selftok_engine* e, Window* win, int B, cudaStream_t s) {
+  DecodeWs& w = e->dws;
+  STK_TRY(upload_plan(e, w.plan, s));
   win->range = w.plan;
   win->plan = w.plan + 2 * B;
   return 0;
@@ -1417,6 +1450,89 @@ static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const floa
     e->last_launches = g->second;
   }
   if (x0_out_dev != w.x_lat) STK_CUDA(cudaMemcpyAsync(x0_out_dev, w.x_lat, sizeof(float) * nlat, cudaMemcpyDeviceToDevice, s));
+  return SELFTOK_OK;
+}
+
+// One Euler step per image at its own schedule row (continuous batching): x_out[b] = x[b] - dt[s_b] v_b, eager, over a packed
+// context stream (see Packed).  Bitwise what selftok_decode(_cfg)(_range) computes for that image at step s_b.
+extern "C" __attribute__((visibility("default"))) int selftok_decode_step(selftok_handle_t e, const int64_t* tokens_dev, const int32_t* range_host,
+                                   const int32_t* step_host, const float* cfg_scale_host, const float* x_dev, int B,
+                                   float* x_out_dev, void* stream) {
+  HOT_PROLOGUE(e);
+  STK_CHECK(tokens_dev && step_host && x_dev && x_out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_decode_step: bad argument");
+  STK_CHECK(!e->cfg.renderer, SELFTOK_ERR_STATE, "selftok_decode_step: handle was created for the renderer");
+  const bool guided = cfg_scale_host != nullptr;
+  STK_CHECK(!guided || e->has_cfg, SELFTOK_ERR_STATE, "selftok_decode_step: guided steps need selftok_set_cfg_schedule before finalize");
+  const selftok_config_t& c = e->cfg;
+  const int K = c.K, N = e->Nimg;
+  // the per-image block, validated before anything is launched
+  std::vector<int>& h = e->plan_host;
+  h.assign((size_t)B * PK_IMG_INTS, 0);
+  int Mc = 0, cmax = 0;
+  for (int b = 0; b < B; ++b) {
+    const int st = step_host[b];
+    if (st < 0 || st >= e->steps) {
+      set_error("selftok_decode_step: step of image " + std::to_string(b) + " is " + std::to_string(st) + ", not in [0, " +
+                std::to_string(e->steps) + ")");
+      return SELFTOK_ERR_BAD_ARG;
+    }
+    const int lo = range_host ? range_host[2 * b] : 0, hi = range_host ? range_host[2 * b + 1] : K;
+    if (!(0 <= lo && lo < hi && hi <= K)) {
+      set_error("selftok_decode_step: token range of image " + std::to_string(b) + ": [" + std::to_string(lo) + ", " +
+                std::to_string(hi) + ") is not a window 0 <= lo < hi <= K = " + std::to_string(K));
+      return SELFTOK_ERR_BAD_ARG;
+    }
+    const int end = hi < e->k[st] + 1 ? hi : e->k[st] + 1;
+    const int cb = end > lo ? end - lo : 0;
+    if (guided && cb == 0) {
+      set_error("selftok_decode_step: image " + std::to_string(b) + " has no visible token at step " + std::to_string(st) +
+                " (the guided sampler needs lo <= k = " + std::to_string(e->k[st]) + ", got lo = " + std::to_string(lo) + ")");
+      return SELFTOK_ERR_BAD_ARG;
+    }
+    h[2 * b] = Mc; h[2 * b + 1] = cb; h[2 * B + b] = lo; h[3 * B + b] = st;
+    memcpy(&h[4 * B + b], &e->dt[st], sizeof(float));
+    if (guided) memcpy(&h[5 * B + b], &cfg_scale_host[b], sizeof(float));
+    Mc += cb;
+    cmax = cb > cmax ? cb : cmax;
+  }
+  STK_TRY(ensure_dws(e, B));
+  DecodeWs& w = e->dws;
+  STK_TRY(upload_plan(e, w.pk, s));
+  int* rows = w.pk + (int64_t)PK_IMG_INTS * B;
+  const int64_t BK = (int64_t)B * K;
+  Packed pk;
+  pk.Mc = Mc; pk.S = cmax + N; pk.pair = w.pk;
+  pk.dt = reinterpret_cast<const float*>(w.pk + 4 * B); pk.scale = reinterpret_cast<const float*>(w.pk + 5 * B);
+  pk.ctx_tok = rows; pk.ctx_pos = rows + BK; pk.ctx_step = rows + 2 * BK; pk.ctx_dst = rows + 3 * BK; pk.x_step = rows + 4 * BK;
+  PROF(PC_OTHER, launch_expand_packed(w.pk, B, K, N, pk.S, rows, rows + BK, rows + 2 * BK, rows + 3 * BK, rows + 4 * BK, s));
+  const int64_t row_bytes = (int64_t)3 * e->D * (tc_mode(e) ? 2 : 4);
+  if (!tc_mode(e)) PROF(PC_OTHER, launch_zero_slot_tails(pk.pair, B, pk.S, N, w.qkv, row_bytes, s));
+  if (w.qkv_hi) PROF(PC_OTHER, launch_zero_slot_tails(pk.pair, B, pk.S, N, w.qkv_hi, row_bytes, s));
+  if (w.qkv_lo) PROF(PC_OTHER, launch_zero_slot_tails(pk.pair, B, pk.S, N, w.qkv_lo, row_bytes, s));
+  if (Mc > 0) {
+    // context_embedder(outs_q) + context_pos_embed of the visible rows only, straight into the context stream
+    STK_TRY(run_lookup(e, tokens_dev, B, w.outs_q, s, nullptr, pk.ctx_tok, Mc));
+    GETW(cp, "model.context_pos_embed");
+    STK_CHECK(cp->numel == (int64_t)K * e->D, SELFTOK_ERR_BAD_ARG, "context_pos_embed shape");
+    Epilogue ep;
+    ep.out = w.ctx; ep.addtab = cp->d; ep.add_ld = e->D; ep.tab_rows = pk.ctx_pos;
+    STK_TRY(lin32(e, "model.context_embedder", w.outs_q, c.code_dim, Mc, ep, s));
+  }
+  PROF(PC_OTHER, launch_patchify(x_dev, w.patch, B, c.in_channels, c.latent, c.latent, c.dit_patch, s));
+  STK_TRY(x_embed(e, B, s));
+  if (!guided) {
+    STK_TRY(joint_blocks(e, B, 0, 0, /*ctx_self=*/c.context_see_xt == 0, s, false, w.o_final, nullptr, 0, &pk));
+  } else {
+    // as dit_forward_cfg: the conditional pass with context rows blind to image keys, then the image stream alone
+    STK_TRY(joint_blocks(e, B, 0, 0, /*ctx_self=*/true, s, false, w.o_final, nullptr, 0, &pk));
+    STK_TRY(x_embed(e, B, s));
+    Packed pu = pk;
+    pu.Mc = 0; pu.S = N;
+    STK_TRY(joint_blocks(e, B, 0, 0, /*ctx_self=*/false, s, /*uncond=*/true, w.o_final_u, nullptr, 0, &pu));
+  }
+  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, x_dev, x_out_dev, 0.f, B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s,
+                                        guided ? w.o_final_u : nullptr, 1.f, pk.dt, guided ? pk.scale : nullptr));
+  e->last_launches = g_launch_count - launches0;
   return SELFTOK_OK;
 }
 

@@ -49,7 +49,7 @@ __device__ __forceinline__ float2 ldg2(const float* p) { return *reinterpret_cas
 // mode branches.
 template <int MODE, bool GELU>
 __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&acc)[ACC], int64_t row0, int64_t M, int col0, int N) {
-  const bool per_row_gate = MODE == EPI_RESID && e.gate && e.gate_period > 1;
+  const bool per_row_gate = MODE == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
   const bool per_row_add = MODE == EPI_STORE && e.addtab;
   const bool fp16 = e.fp16 != 0;
   int orow[2], mrow[2];
@@ -59,14 +59,17 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&a
     const int64_t m = row0 + 8 * r;
     rvalid[r] = m < M;
     const int mi = (int)m;
-    if (e.plan && rvalid[r]) {                          // token-range plan: image rows per slot = rpb_out - Kc
+    if (e.row_map && rvalid[r]) {
+      orow[r] = e.row_map[mi];
+    } else if (e.plan && rvalid[r]) {                   // token-range plan: image rows per slot = rpb_out - Kc
       const int b = mi / e.rpb_in;
       const int n_img = e.rpb_out - (e.plan_ctx ? e.rpb_in : e.row_off);
       orow[r] = b * e.rpb_out + plan_slot_row(mi % e.rpb_in, e.plan[2 * b], e.plan[2 * b + 1], n_img, e.plan_ctx != 0);
     } else {
       orow[r] = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
     }
-    mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
+    if (e.tab_rows && rvalid[r]) mrow[r] = e.tab_rows[mi];
+    else mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
   }
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {

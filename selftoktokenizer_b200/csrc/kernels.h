@@ -15,6 +15,8 @@ namespace stk {
 // [a_b, a_b + c_b).  The image's slot of rpb_out rows then holds its live context rows, its image rows, and last its other
 // context rows (computed, never visible): plan_ctx = 1 (context stream, rpb_in = Kc): row r -> r - a_b when live, else the tail;
 // plan_ctx = 0 (image stream, rpb_in = N): row r -> c_b + r.
+// Per-row indices (packed step calls, NULL otherwise): tab_rows[m] replaces m % period as the gate / addtab row, and row_map[m]
+// replaces the remap above as the output row.
 enum EpiMode { EPI_STORE = 0, EPI_RESID = 1, EPI_SPLIT = 2 };
 struct Epilogue {
   int mode = EPI_STORE;
@@ -35,6 +37,8 @@ struct Epilogue {
   int fp16 = 0;                          // EPI_SPLIT: planes hold IEEE half (single-pass fp16 mode) instead of bf16
   const int* plan = nullptr;             // token-range plan of this step, [B][2] int32 (a, c); NULL: plain remap
   int plan_ctx = 0;
+  const int* tab_rows = nullptr;         // [M] gate (EPI_RESID) / addtab (EPI_STORE) row of GEMM row m
+  const int* row_map = nullptr;          // [M] output row of GEMM row m
 };
 // slot row of stream row r of an image with plan pair (a, c); n_img = image rows per slot
 __host__ __device__ __forceinline__ int plan_slot_row(int r, int a, int c, int n_img, bool ctx) {
@@ -45,10 +49,11 @@ __host__ __device__ __forceinline__ int plan_slot_row(int r, int a, int c, int n
 // ---- fp32 FFMA kernels (kernels_simt.cu) ---------------------------------------------------------------------
 int launch_linear_f32(const float* A, int64_t lda, const float* W, int64_t ldw, int64_t M, int N, int K,
                       const Epilogue& ep, cudaStream_t s);
-// LN (no affine, eps) + modulate; writes fp32 and/or bf16 planes.  shift/scale NULL -> plain LN.
+// LN (no affine, eps) + modulate; writes fp32 and/or bf16 planes.  shift/scale NULL -> plain LN.  rows != NULL: row m uses
+// table row rows[m] instead of m % period.
 int launch_ln_mod(const float* x, int64_t ldx, const float* shift, const float* scale, int64_t ld_mod, int period,
                   float* out_f32, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, int64_t ldo, int64_t M, int D,
-                  float eps, cudaStream_t s, int fp16 = 0);
+                  float eps, cudaStream_t s, int fp16 = 0, const int* rows = nullptr);
 // Two LN + modulate problems (the context- and the image-row pass of one MMDiT layer stage) in ONE launch, 16-bit plane
 // output (IEEE half when fp16, else bf16 hi [+ lo]).  period > 1: rows are [image][position] with a per-position table row
 // (M must be a multiple of period); period <= 1: one table row for all rows.
@@ -61,6 +66,7 @@ struct LnProblem {
   __nv_bfloat16* out_hi = nullptr;
   __nv_bfloat16* out_lo = nullptr;
   int64_t M = 0;
+  const int* rows = nullptr;         // [M] table row of every row (packed step calls; then for every problem of the launch)
   int imgs = 0;                      // filled by the launcher
 };
 int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStream_t s, int fp16);
@@ -78,11 +84,14 @@ struct AttnOut {
 // then its S - c_b - n_img other context rows (see Epilogue).  Image rows see keys [0, c_b + n_img); context rows the same, or
 // [0, c_b) with ctx_self; a row with no visible key writes 0.  route != 0: output rows go back to the streams (inverse of the
 // QKV remap; AttnOut.split = Kc = S - n_img), else AttnOut's own routing applies.
+// packed: the plan pairs are (off_b, c_b) of a packed context stream (selftok_decode_step): slot row r < c_b goes to context row
+// off_b + r, image rows to b * n_img + r - c_b; rows >= c_b + n_img hold nothing and are not written.
 struct AttnPlan {
   const int* plan = nullptr;             // [B][2] int32 (a, c) of this step
   int n_img = 0;
   int ctx_self = 0;
   int route = 1;
+  int packed = 0;
 };
 // stream row of slot row `row` of an image with plan pair (a, c); ctx = whether it is a context row
 __host__ __device__ __forceinline__ int plan_stream_row(int row, int a, int c, int n_img, bool& ctx) {
@@ -103,16 +112,26 @@ int launch_vq(const float* z, int64_t R, int Q, const float* w_in, const float* 
               const float* codebook_t, int n_codes, int code_dim, const float* ln_w, const float* ln_b,
               int64_t* ids, float* outs_q, cudaStream_t s);
 // ids outside [0, n_codes): row poisoned with NaN and counted in *bad_ids (may be NULL).  range != NULL: [R / K][2] int32 (lo, hi)
-// token windows; positions outside an image's window are not read and write a zero row.
+// token windows; positions outside an image's window are not read and write a zero row.  gather != NULL: output row m reads
+// ids[gather[m]] (packed context stream).
 int launch_lookup_ln3(const int64_t* ids, int64_t R, const float* codebook, int n_codes, int code_dim,
                       const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s,
-                      const int* range = nullptr, int K = 0);
+                      const int* range = nullptr, int K = 0, const int* gather = nullptr);
 // [B,C,Hh,Ww] latents -> [B*(Hh/p)*(Ww/p), C*p*p] patch rows ((c,ph,pw) fastest-last, Conv2d weight order)
 int launch_patchify(const float* x, float* out, int B, int C, int Hh, int Ww, int p, cudaStream_t s);
 // x_lat[b,c,h*p+ph,w*p+pw] = x_in[...] - dt * o[b, h*g+w, (ph*p+pw)*C + c]   (unpatchify + Euler; dt = -1 & x_in NULL: plain unpatchify)
-// o_u != NULL (guided sampler): v = o_u + cfg_scale * (o - o_u) first
+// o_u != NULL (guided sampler): v = o_u + cfg_scale * (o - o_u) first.  dt_img / scale_img != NULL: device [B] per-image dt and
+// cfg_scale instead of the scalars
 int launch_unpatchify_axpy(const float* o, const float* x_in, float* x_out, float dt, int B, int C, int g, int p,
-                           cudaStream_t s, const float* o_u = nullptr, float cfg_scale = 1.f);
+                           cudaStream_t s, const float* o_u = nullptr, float cfg_scale = 1.f, const float* dt_img = nullptr,
+                           const float* scale_img = nullptr);
+// Per-row maps of a packed step call from its per-image block blk = [B][2] (off_b, c_b) | [B] lo_b | [B] step_b: context row
+// m = off_b + r (r < c_b) gets ctx_tok = b K + lo_b + r, ctx_pos = lo_b + r, ctx_step = step_b, ctx_dst = b S + r; image row
+// b N + r gets x_step = step_b.
+int launch_expand_packed(const int* blk, int B, int K, int N, int S, int* ctx_tok, int* ctx_pos, int* ctx_step, int* ctx_dst,
+                         int* x_step, cudaStream_t s);
+// zero the rows [c_b + n_img, S) of slot b up to its next 64-row boundary (pair = [B][2] (off_b, c_b)) in a [B*S] x row_bytes buffer
+int launch_zero_slot_tails(const int* pair, int B, int S, int n_img, void* buf, int64_t row_bytes, cudaStream_t s);
 int launch_transpose(const float* in, float* out, int rows, int cols, cudaStream_t s);
 int launch_split_bf16(const float* in, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, cudaStream_t s, int fp16 = 0);
 // out[b, r, :] = src[r, :] for b in 0..B-1 (broadcast rows), optionally + add[r,:]

@@ -115,7 +115,10 @@ __global__ void __launch_bounds__(256, 2) linear_f32_kernel(const LinParams p) {
     const int64_t m = m0 + (i / 4) * (BM / CM) + ty * 4 + (i % 4);
     if (m >= p.M) continue;
     int64_t orow = m;
-    if (e.plan) {                                           // token-range plan: image rows per slot = rpb_out - Kc
+    const int64_t trow_m = e.tab_rows ? e.tab_rows[m] : m;  // gate / addtab row before the period wrap
+    if (e.row_map) {
+      orow = e.row_map[m];
+    } else if (e.plan) {                                    // token-range plan: image rows per slot = rpb_out - Kc
       const int b = (int)(m / e.rpb_in);
       const int n_img = e.rpb_out - (e.plan_ctx ? e.rpb_in : e.row_off);
       orow = (int64_t)b * e.rpb_out + plan_slot_row((int)(m % e.rpb_in), e.plan[2 * b], e.plan[2 * b + 1], n_img, e.plan_ctx != 0);
@@ -134,10 +137,10 @@ __global__ void __launch_bounds__(256, 2) linear_f32_kernel(const LinParams p) {
         if (e.bias) y += e.bias[nn];
         y = apply_act(y, e.act);
         if (e.mode == EPI_STORE) {
-          if (e.addtab) y += e.addtab[(m % e.add_period) * e.add_ld + nn];
+          if (e.addtab) y += e.addtab[(e.tab_rows ? trow_m : m % e.add_period) * e.add_ld + nn];
           e.out[orow * e.ldo + nn] = y;
         } else if (e.mode == EPI_RESID) {
-          float g = e.gate ? e.gate[(m % e.gate_period) * e.gate_ld + nn] : 1.0f;
+          float g = e.gate ? e.gate[(e.tab_rows ? trow_m : m % e.gate_period) * e.gate_ld + nn] : 1.0f;
           e.out[orow * e.ldo + nn] = e.resid[orow * e.ldo + nn] + g * y;
         } else {
           uint16_t hi, lo;
@@ -184,7 +187,8 @@ __global__ void __launch_bounds__(256) ln_mod_kernel(const float* __restrict__ x
                                                      const float* __restrict__ shift, const float* __restrict__ scale,
                                                      int64_t ld_mod, int period, float* __restrict__ out_f32,
                                                      __nv_bfloat16* __restrict__ out_hi, __nv_bfloat16* __restrict__ out_lo,
-                                                     int64_t ldo, int64_t M, int D, float eps, int fp16, int imgs) {
+                                                     int64_t ldo, int64_t M, int D, float eps, int fp16, int imgs,
+                                                     const int* __restrict__ rows) {
   __shared__ __align__(16) float4 tab[STAGED ? 2 * MAXV * 32 : 1];     // [shift | scale] of the CTA's table row
   const int lane = threadIdx.x & 31;
   const int nv = D >> 2;                              // float4 per row
@@ -242,7 +246,7 @@ __global__ void __launch_bounds__(256) ln_mod_kernel(const float* __restrict__ x
     __syncthreads();
     if (!active) return;
   } else if (shift) {
-    const int64_t mrow = (period > 0) ? (m % period) : 0;
+    const int64_t mrow = rows ? rows[m] : (period > 0) ? (m % period) : 0;
     sh = reinterpret_cast<const float4*>(shift + mrow * ld_mod);
     sc = reinterpret_cast<const float4*>(scale + mrow * ld_mod);
   }
@@ -270,18 +274,19 @@ __global__ void __launch_bounds__(256) ln_mod_kernel(const float* __restrict__ x
 
 int launch_ln_mod(const float* x, int64_t ldx, const float* shift, const float* scale, int64_t ld_mod, int period,
                   float* out_f32, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, int64_t ldo, int64_t M, int D,
-                  float eps, cudaStream_t s, int fp16) {
+                  float eps, cudaStream_t s, int fp16, const int* rows) {
   STK_CHECK(x && M > 0 && D > 0 && D % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0 && ld_mod % 4 == 0, -1, "ln_mod: bad arguments");
+  STK_CHECK(!rows || shift, -1, "ln_mod: per-row table indices without a table");
   STK_CHECK((shift == nullptr) == (scale == nullptr), -1, "ln_mod: shift and scale must both be given or both NULL");
   STK_CHECK(D <= 2048, -2, "ln_mod: D > 2048 unsupported");
   const int wpb = 8;
   // position-major mapping when the rows are [image][position] with per-position tables (see the kernel comment)
-  const int imgs = (period > 1 && shift && M % period == 0 && M / period >= 2) ? (int)(M / period) : 0;
+  const int imgs = (!rows && period > 1 && shift && M % period == 0 && M / period >= 2) ? (int)(M / period) : 0;
   dim3 grid(imgs ? (unsigned)(period * ((imgs + wpb - 1) / wpb)) : (unsigned)((M + wpb - 1) / wpb));
-  const bool staged = shift && (imgs > 0 || period <= 1);            // one table row per CTA
+  const bool staged = shift && !rows && (imgs > 0 || period <= 1);   // one table row per CTA
 #define STK_LN(MAXV, ST)                                                                                                      \
   ln_mod_kernel<MAXV, ST><<<grid, wpb * 32, 0, s>>>(x, ldx, shift, scale, ld_mod, period, out_f32, out_hi, out_lo, ldo, M, D, eps, \
-                                                    fp16, imgs)
+                                                    fp16, imgs, rows)
   if (D <= 512) { if (staged) STK_LN(4, true); else STK_LN(4, false); }
   else if (D <= 1536) { if (staged) STK_LN(12, true); else STK_LN(12, false); }
   else { if (staged) STK_LN(16, true); else STK_LN(16, false); }
@@ -306,7 +311,9 @@ struct LnPairParams {
 // FULL: D == MAXV * 128 exactly (1536 with MAXV 12: the MMDiT), so that no per-chunk bounds predicate is compiled in.
 // ROWS: rows per warp (the CTA covers 8 * ROWS rows that share one table row): the prologue -- index arithmetic, the staged table,
 // the CTA launch itself -- is ~370 of the ~590 instructions a warp spends on its first row.
-template <int MAXV, bool FP16, bool LO, bool FULL, int ROWS>
+// GATHER: every row reads its own table row rows[m] from global memory (packed step calls: rows of one CTA sit at different
+// schedule rows or positions); the arithmetic is the same.
+template <int MAXV, bool FP16, bool LO, bool FULL, int ROWS, bool GATHER>
 __global__ void __launch_bounds__(256) ln_mod_pair_kernel(const LnPairParams p) {
   __shared__ __align__(16) float4 tab[2 * MAXV * 32];
   const bool second = (int)blockIdx.x >= p.nblk0;
@@ -320,7 +327,7 @@ __global__ void __launch_bounds__(256) ln_mod_pair_kernel(const LnPairParams p) 
   const int64_t first = pos_major ? (int64_t)(blk / q.period) * (8 * ROWS) + wid : (int64_t)blk * (8 * ROWS) + wid;
   const int64_t trow = pos_major ? blk % q.period : 0;
   const int64_t limit = pos_major ? q.imgs : q.M;
-  {
+  if (!GATHER) {
     const float4* sh = reinterpret_cast<const float4*>(q.shift + trow * q.ld_mod);
     const float4* sc = reinterpret_cast<const float4*>(q.scale + trow * q.ld_mod);
     for (int t = threadIdx.x; t < nv; t += 256) {
@@ -374,11 +381,13 @@ __global__ void __launch_bounds__(256) ln_mod_pair_kernel(const LnPairParams p) 
     if (!active) continue;
     uint2* oh = reinterpret_cast<uint2*>(q.out_hi + m * (int64_t)p.D);
     uint2* ol = LO ? reinterpret_cast<uint2*>(q.out_lo + m * (int64_t)p.D) : nullptr;
+    const float4* gsh = GATHER ? reinterpret_cast<const float4*>(q.shift + (int64_t)q.rows[m] * q.ld_mod) : nullptr;
+    const float4* gsc = GATHER ? reinterpret_cast<const float4*>(q.scale + (int64_t)q.rows[m] * q.ld_mod) : nullptr;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) {
       const int idx = lane + i * 32;
       if (FULL || idx < nv) {
-        const float4 h4 = tab[idx], s4 = tab[MAXV * 32 + idx];
+        const float4 h4 = GATHER ? gsh[idx] : tab[idx], s4 = GATHER ? gsc[idx] : tab[MAXV * 32 + idx];
         float4 y, g;
         ffma2(v[i].x, v[i].y, rstd, rstd, nmr, nmr, y.x, y.y);
         ffma2(v[i].z, v[i].w, rstd, rstd, nmr, nmr, y.z, y.w);
@@ -413,14 +422,16 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
     }
     return c;
   };
-  const int rows = ctas_for(2) >= 4 * sms ? 2 : 1;
+  const bool gather = probs[0].rows != nullptr;
+  const int rows = !gather && ctas_for(2) >= 4 * sms ? 2 : 1;
   for (int i = 0; i < 2; ++i) {
     if (i >= n) { p.pr[i] = probs[0]; p.pr[i].M = 0; continue; }
     LnProblem q = probs[i];
     STK_CHECK(q.x && q.shift && q.scale && q.out_hi && q.M > 0 && q.ld_mod % 4 == 0, -1, "ln_mod_pair: bad problem");
     STK_CHECK(i == 0 || (q.out_lo != nullptr) == lo, -1, "ln_mod_pair: both problems must use the same plane set");
     lo = q.out_lo != nullptr;
-    if (q.period > 1) {                                // per-position table: position-major, needs whole images
+    STK_CHECK((q.rows != nullptr) == gather, -1, "ln_mod_pair: per-row table indices must be given for both problems or neither");
+    if (q.period > 1 && !gather) {                                // per-position table: position-major, needs whole images
       STK_CHECK(q.M % q.period == 0, -1, "ln_mod_pair: rows must be whole images of `period` positions");
       q.imgs = (int)(q.M / q.period);
       nblk[i] = q.period * ((q.imgs + 8 * rows - 1) / (8 * rows));
@@ -433,19 +444,19 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
   STK_CHECK(!(fp16 && lo), -1, "ln_mod_pair: the fp16 mode has no residual planes");
   p.nblk0 = nblk[0];
   const unsigned grid = (unsigned)(nblk[0] + nblk[1]);
-#define STK_LNP3(MAXV, FULL, ROWS)                                                          \
-  do {                                                                                      \
-    if (fp16) ln_mod_pair_kernel<MAXV, true, false, FULL, ROWS><<<grid, 256, 0, s>>>(p);    \
-    else if (lo) ln_mod_pair_kernel<MAXV, false, true, FULL, ROWS><<<grid, 256, 0, s>>>(p); \
-    else ln_mod_pair_kernel<MAXV, false, false, FULL, ROWS><<<grid, 256, 0, s>>>(p);        \
+#define STK_LNP3(MAXV, FULL, ROWS, G)                                                          \
+  do {                                                                                         \
+    if (fp16) ln_mod_pair_kernel<MAXV, true, false, FULL, ROWS, G><<<grid, 256, 0, s>>>(p);    \
+    else if (lo) ln_mod_pair_kernel<MAXV, false, true, FULL, ROWS, G><<<grid, 256, 0, s>>>(p); \
+    else ln_mod_pair_kernel<MAXV, false, false, FULL, ROWS, G><<<grid, 256, 0, s>>>(p);        \
   } while (0)
-#define STK_LNP(MAXV)                                                                       \
-  do {                                                                                      \
-    if (D == MAXV * 128) {                                                                  \
-      if (rows == 2) STK_LNP3(MAXV, true, 2); else STK_LNP3(MAXV, true, 1);                 \
-    } else {                                                                                \
-      if (rows == 2) STK_LNP3(MAXV, false, 2); else STK_LNP3(MAXV, false, 1);               \
-    }                                                                                       \
+#define STK_LNP(MAXV)                                                                                                      \
+  do {                                                                                                                     \
+    if (D == MAXV * 128) {                                                                                                 \
+      if (gather) STK_LNP3(MAXV, true, 1, true); else if (rows == 2) STK_LNP3(MAXV, true, 2, false); else STK_LNP3(MAXV, true, 1, false); \
+    } else {                                                                                                               \
+      if (gather) STK_LNP3(MAXV, false, 1, true); else if (rows == 2) STK_LNP3(MAXV, false, 2, false); else STK_LNP3(MAXV, false, 1, false); \
+    }                                                                                                                      \
   } while (0)
   if (D <= 512) STK_LNP(4);
   else if (D <= 1536) STK_LNP(12);
@@ -498,6 +509,7 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
   }
   // keys a row may see (token-range plan: this image's live context rows pc and live keys [0, live), see AttnPlan)
   const int pc = p.pl.plan ? p.pl.plan[2 * b + 1] : 0, live = p.pl.plan ? pc + p.pl.n_img : Sk;
+  if (p.pl.packed && q0 >= live) return;                         // packed slot: no row of this tile holds anything
   int kmax_row[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -642,7 +654,11 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const AttnParams p) 
     const AttnOut& t = p.out;
     bool inA = row < t.split;
     int64_t orow = inA ? ((int64_t)b * t.split + row) : ((int64_t)b * (p.Sq - t.split) + (row - t.split));
-    if (p.pl.plan && p.pl.route) {
+    if (p.pl.packed) {
+      if (row >= live) continue;
+      inA = row < pc;
+      orow = inA ? (int64_t)p.pl.plan[2 * b] + row : (int64_t)b * p.pl.n_img + row - pc;
+    } else if (p.pl.plan && p.pl.route) {
       const int sr = plan_stream_row(row, p.pl.plan[2 * b], pc, p.pl.n_img, inA);
       orow = inA ? (int64_t)b * t.split + sr : (int64_t)b * p.pl.n_img + sr;
     }
@@ -900,7 +916,8 @@ int launch_vq(const float* z, int64_t R, int Q, const float* w_in, const float* 
 // host-buffer entry points return SELFTOK_ERR_BAD_ARG).  Nothing is clamped silently.
 __global__ void lookup_ln3_kernel(const int64_t* __restrict__ ids, int64_t R, const float* __restrict__ codebook,
                                   int n_codes, int dim, const float* __restrict__ ln_w, const float* __restrict__ ln_b,
-                                  float* __restrict__ outs_q, int* __restrict__ bad_ids, const int* __restrict__ range, int K) {
+                                  float* __restrict__ outs_q, int* __restrict__ bad_ids, const int* __restrict__ range, int K,
+                                  const int* __restrict__ gather) {
   const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= R) return;
   if (range) {                                                  // token window: positions outside it are not read
@@ -910,7 +927,7 @@ __global__ void lookup_ln3_kernel(const int64_t* __restrict__ ids, int64_t R, co
       return;
     }
   }
-  const int64_t id = ids[row];
+  const int64_t id = ids[gather ? (int64_t)gather[row] : row];
   if (id < 0 || id >= n_codes) {
     if (bad_ids) atomicAdd(bad_ids, 1);
     for (int d = 0; d < dim; ++d) outs_q[row * dim + d] = __int_as_float(0x7fc00000);
@@ -926,11 +943,13 @@ __global__ void lookup_ln3_kernel(const int64_t* __restrict__ ids, int64_t R, co
 }
 
 int launch_lookup_ln3(const int64_t* ids, int64_t R, const float* codebook, int n_codes, int code_dim,
-                      const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s, const int* range, int K) {
+                      const float* ln_w, const float* ln_b, float* outs_q, int* bad_ids, cudaStream_t s, const int* range, int K,
+                      const int* gather) {
   STK_CHECK(ids && codebook && ln_w && ln_b && outs_q && R > 0, -1, "lookup: bad arguments");
+  STK_CHECK(!(range && gather), -1, "lookup: token windows and a gather map are exclusive");
   STK_CHECK(!range || (K > 0 && R % K == 0), -1, "lookup: token windows need whole images");
   lookup_ln3_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(ids, R, codebook, n_codes, code_dim, ln_w, ln_b, outs_q, bad_ids,
-                                                                range, K);
+                                                                range, K, gather);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;
@@ -960,7 +979,8 @@ int launch_patchify(const float* x, float* out, int B, int C, int Hh, int Ww, in
 // x_prev = x - (a_t - a_prev) * v (sd3/rectified_flow.py:303).
 // Guided sampler (rectified_flow.py:280-289): with o_u the velocity is  v = v_u + cfg_scale * (v_c - v_u)  before the update.
 __global__ void unpatchify_axpy_kernel(const float* __restrict__ o, const float* __restrict__ x_in, float* __restrict__ x_out,
-                                       float dt, int B, int C, int g, int p, const float* __restrict__ o_u, float cfg_scale) {
+                                       float dt, int B, int C, int g, int p, const float* __restrict__ o_u, float cfg_scale,
+                                       const float* __restrict__ dt_img, const float* __restrict__ scale_img) {
   const int Hh = g * p;
   const int64_t total = (int64_t)B * C * Hh * Hh;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -968,16 +988,59 @@ __global__ void unpatchify_axpy_kernel(const float* __restrict__ o, const float*
     int yh = (int)(t % Hh); t /= Hh; int c = (int)(t % C); int b = (int)(t / C);
     int h = yh / p, ph = yh % p, w = xw / p, pw = xw % p;
     const int64_t oi = ((int64_t)b * g * g + h * g + w) * (p * p * C) + (ph * p + pw) * C + c;
+    const float dtb = dt_img ? dt_img[b] : dt, csb = scale_img ? scale_img[b] : cfg_scale;
     float v = o[oi];
-    if (o_u) { const float vu = o_u[oi]; v = vu + cfg_scale * (v - vu); }
-    x_out[i] = x_in ? (x_in[i] - dt * v) : v;
+    if (o_u) { const float vu = o_u[oi]; v = vu + csb * (v - vu); }
+    x_out[i] = x_in ? (x_in[i] - dtb * v) : v;
   }
 }
 int launch_unpatchify_axpy(const float* o, const float* x_in, float* x_out, float dt, int B, int C, int g, int p,
-                           cudaStream_t s, const float* o_u, float cfg_scale) {
+                           cudaStream_t s, const float* o_u, float cfg_scale, const float* dt_img, const float* scale_img) {
   STK_CHECK(o && x_out, -1, "unpatchify: bad arguments");
   int64_t total = (int64_t)B * C * g * p * g * p;
-  unpatchify_axpy_kernel<<<(unsigned)((total + 255) / 256 > 4096 ? 4096 : (total + 255) / 256), 256, 0, s>>>(o, x_in, x_out, dt, B, C, g, p, o_u, cfg_scale);
+  unpatchify_axpy_kernel<<<(unsigned)((total + 255) / 256 > 4096 ? 4096 : (total + 255) / 256), 256, 0, s>>>(o, x_in, x_out, dt, B, C, g, p, o_u, cfg_scale,
+                                                                                                           dt_img, scale_img);
+  count_launch();
+  STK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+__global__ void expand_packed_kernel(const int* __restrict__ blk, int B, int K, int N, int S, int* __restrict__ ctx_tok,
+                                     int* __restrict__ ctx_pos, int* __restrict__ ctx_step, int* __restrict__ ctx_dst,
+                                     int* __restrict__ x_step) {
+  const int b = blockIdx.y, r = blockIdx.x * blockDim.x + threadIdx.x;
+  const int off = blk[2 * b], c = blk[2 * b + 1], lo = blk[2 * B + b], step = blk[3 * B + b];
+  if (r < c) {
+    const int m = off + r;
+    ctx_tok[m] = b * K + lo + r;
+    ctx_pos[m] = lo + r;
+    ctx_step[m] = step;
+    ctx_dst[m] = b * S + r;
+  }
+  if (r < N) x_step[b * N + r] = step;
+}
+int launch_expand_packed(const int* blk, int B, int K, int N, int S, int* ctx_tok, int* ctx_pos, int* ctx_step, int* ctx_dst,
+                         int* x_step, cudaStream_t s) {
+  STK_CHECK(blk && B > 0 && K > 0 && N > 0 && S >= N, -1, "expand_packed: bad arguments");
+  const int n = K > N ? K : N;
+  expand_packed_kernel<<<dim3((unsigned)((n + 127) / 128), (unsigned)B), 128, 0, s>>>(blk, B, K, N, S, ctx_tok, ctx_pos, ctx_step, ctx_dst,
+                                                                                       x_step);
+  count_launch();
+  STK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// zeroes slot rows [c_b + N, min(S, c_b + N rounded up to 64)): the keys the attention loads with the last visible ones (masked, but a
+// stale non-finite value times a zero weight would still reach the output)
+__global__ void zero_slot_tails_kernel(const int* __restrict__ pair, int S, int N, char* __restrict__ buf, int64_t row_bytes) {
+  const int b = blockIdx.y, r0 = pair[2 * b + 1] + N, r = r0 + blockIdx.x;
+  if (r >= S || r >= (r0 + 63) / 64 * 64) return;
+  uint32_t* row = reinterpret_cast<uint32_t*>(buf + ((int64_t)b * S + r) * row_bytes);
+  for (int64_t t = threadIdx.x; t < row_bytes / 4; t += blockDim.x) row[t] = 0u;
+}
+int launch_zero_slot_tails(const int* pair, int B, int S, int N, void* buf, int64_t row_bytes, cudaStream_t s) {
+  STK_CHECK(pair && buf && B > 0 && S >= N && row_bytes % 4 == 0, -1, "zero_slot_tails: bad arguments");
+  zero_slot_tails_kernel<<<dim3(63, (unsigned)B), 256, 0, s>>>(pair, S, N, reinterpret_cast<char*>(buf), row_bytes);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;

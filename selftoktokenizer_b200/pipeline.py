@@ -349,20 +349,30 @@ class SelftokPipeline:
         print("Begin decoding.")
         self._need_vae()
         pred_x0 = self.decode_latents(idx, token_range=token_range)
+        recons = self._latents_to_pixels(pred_x0)
+        print("End decoding.")
+        return recons
+
+    def _latents_to_pixels(self, pred_x0: torch.Tensor) -> torch.Tensor:
+        """The tail of decoding(): sampler latents -> VAE latent space -> pixels in [0, 1] (SelftokPipeline.py:272-276)."""
         pred_x0_out = SD3LatentFormat().process_out(pred_x0).to(self.dtype)
         recons = self.vae.decode(pred_x0_out, return_dict=False)[0]
         norm_ip(recons, -1, 1)
-        print("End decoding.")
         return recons
+
+    def continuous_decoder(self, max_batch: int = 64, *, guided: bool = False):
+        """A `ContinuousDecoder` over this pipeline's engine: requests join the running batch at any sampler step and leave when
+        their own steps are done; each result is the pixels decoding() gives for that image alone (same noise draw)."""
+        from .continuous import ContinuousDecoder
+        self._need_vae()
+        return ContinuousDecoder(self.engine, max_batch, guided=guided, postprocess=torch.no_grad()(self._latents_to_pixels))
 
     @torch.no_grad()
     def decoding_cfg(self, idx, device, cfg_scale: Optional[float] = None, *, token_range=None):
         """decoding() with the guided sampler (cfg_scale defaults to the constructor's); token_range as in `decode_latents`."""
         self._need_vae()
         pred_x0 = self.decode_latents(idx, cfg_scale=self.cfg_scale if cfg_scale is None else cfg_scale, token_range=token_range)
-        recons = self.vae.decode(SD3LatentFormat().process_out(pred_x0).to(self.dtype), return_dict=False)[0]
-        norm_ip(recons, -1, 1)
-        return recons
+        return self._latents_to_pixels(pred_x0)
 
     @torch.no_grad()
     def decoding_with_renderer(self, idx, device, *, token_range=None):
