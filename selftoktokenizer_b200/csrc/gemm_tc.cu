@@ -4,7 +4,7 @@
 //              y = A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T, all three products accumulated into the same registers.
 //   tile       128 x 256 x 64 per pipeline stage per CTA; two consumer warpgroups, each wgmma m64n256k16 on its 64 rows
 //   staging    TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared memory ring, mbarrier full/empty pairs
-//   roles      warpgroups 0-1: wgmma + epilogue (registers -> HBM) | warp 8: TMA producer (1 thread)
+//   roles      warpgroups 0-1: wgmma + epilogue (registers -> HBM) | warpgroup 2: TMA producer (1 thread)
 //   cluster    CL == 2: two CTAs (rows 256 apart in M) share the W tile: each loads half of it and multicasts it to both,
 //              halving the L2 -> SM traffic of the weights; CL == 1: one CTA loads the whole tile
 //   schedule   persistent CTAs (grid = #SMs), tiles rasterised in groups of M-blocks for L2 reuse of W
@@ -27,8 +27,12 @@ constexpr int BM = 128, BN = 256, BK = 64, WK = 16;
 constexpr int A_TILE_BYTES = BM * BK * 2;      // 16 KiB
 constexpr int B_TILE_BYTES = BN * BK * 2;      // 32 KiB
 constexpr int CONSUMERS = 2;                   // warpgroups of 64 rows
-constexpr int NUM_THREADS = CONSUMERS * 128 + 32;
+constexpr int NUM_THREADS = CONSUMERS * 128 + 128;  // + one producer warpgroup (one thread of it issues the TMA loads)
+// Register split (setmaxnreg): 2 x 128 x 232 + 128 x 40 = 64,512 of the 65,536 registers.  The consumers hold 128 fp32
+// accumulators plus a batch of epilogue operands; at the 168 registers an even split leaves them, the epilogue spills.
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr int ACC = BN / 2;                    // fp32 accumulators per consumer thread
+constexpr int kPrefetchKBlocks = 4;            // residual rows go to L2 this many k-blocks before the epilogue
 
 template <int NSPLIT> struct Cfg {
   static constexpr int PLANES = NSPLIT == 3 ? 2 : 1;
@@ -44,77 +48,125 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[ACC], uint64_t da, uint64_
 
 __device__ __forceinline__ float2 ldg2(const float* p) { return *reinterpret_cast<const float2*>(p); }
 
-// Epilogue of one consumer thread's accumulators: rows row0 and row0 + 8, column pairs col0 + 8 j (j < 32).  Every access of
-// a quad of lanes covers 32 contiguous bytes of a row.  MODE / GELU are compile-time so that the per-element path carries no
-// mode branches.
-template <int MODE, bool GELU>
-__device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&acc)[ACC], int64_t row0, int64_t M, int col0, int N) {
-  const bool per_row_gate = MODE == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
-  const bool per_row_add = MODE == EPI_STORE && e.addtab;
-  const bool fp16 = e.fp16 != 0;
+// Rows of one consumer thread's accumulators (row0 and row0 + 8): output row (token-range plan, packed row_map or the plain
+// [image][row] remap) and gate / addtab table row.  Resolved at tile start, so that the row_map / tab_rows reads and the L2
+// prefetch of the residual rows (epilogue_prefetch) overlap the mainloop.
+struct EpiRows {
   int orow[2], mrow[2];
-  bool rvalid[2];
+  bool valid[2];
+};
+
+__device__ __forceinline__ EpiRows epilogue_rows(const Epilogue& e, int64_t row0, int64_t M) {
+  const bool per_row_gate = e.mode == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
+  const bool per_row_add = e.mode == EPI_STORE && e.addtab;
+  EpiRows rw;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int64_t m = row0 + 8 * r;
-    rvalid[r] = m < M;
+    rw.valid[r] = m < M;
     const int mi = (int)m;
-    if (e.row_map && rvalid[r]) {
-      orow[r] = e.row_map[mi];
-    } else if (e.plan && rvalid[r]) {                   // token-range plan: image rows per slot = rpb_out - Kc
+    rw.orow[r] = 0;
+    if (e.row_map && rw.valid[r]) {
+      rw.orow[r] = e.row_map[mi];
+    } else if (e.plan && rw.valid[r]) {                 // token-range plan: image rows per slot = rpb_out - Kc
       const int b = mi / e.rpb_in;
       const int n_img = e.rpb_out - (e.plan_ctx ? e.rpb_in : e.row_off);
-      orow[r] = b * e.rpb_out + plan_slot_row(mi % e.rpb_in, e.plan[2 * b], e.plan[2 * b + 1], n_img, e.plan_ctx != 0);
-    } else {
-      orow[r] = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
+      rw.orow[r] = b * e.rpb_out + plan_slot_row(mi % e.rpb_in, e.plan[2 * b], e.plan[2 * b + 1], n_img, e.plan_ctx != 0);
+    } else if (rw.valid[r]) {
+      rw.orow[r] = e.rpb_in > 0 ? (mi / e.rpb_in) * e.rpb_out + e.row_off + (mi % e.rpb_in) : mi;
     }
-    if (e.tab_rows && rvalid[r]) mrow[r] = e.tab_rows[mi];
-    else mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
+    if (e.tab_rows && rw.valid[r]) rw.mrow[r] = e.tab_rows[mi];
+    else rw.mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
   }
+  return rw;
+}
+
+// Residual rows of the tile into L2, a few k-blocks before the epilogue reads them: lane q of each quad takes 128 B lines
+// 2q and 2q + 1 of the 1 KB row segment of both its rows.  Only rows < M and columns < N are touched.
+__device__ __forceinline__ void epilogue_prefetch(const Epilogue& e, const EpiRows& rw, int col0, int N) {
+  if (e.mode != EPI_RESID) return;
+  const int c0 = col0 & ~(BN - 1);
+  const int q = (col0 >> 1) & 3;
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int n = col0 + 8 * j;
-    if (n >= N) continue;                               // N % 4 == 0 and n even: a pair is all in or all out
-    const float2 bias = e.bias ? ldg2(e.bias + n) : make_float2(0.f, 0.f);
-    const float2 g0 = (MODE == EPI_RESID && e.gate && !per_row_gate) ? ldg2(e.gate + n) : make_float2(1.f, 1.f);
+  for (int r = 0; r < 2; ++r) {
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      if (!rvalid[r]) continue;
-      float2 y = make_float2(acc[4 * j + 2 * r] + bias.x, acc[4 * j + 2 * r + 1] + bias.y);
-      if (GELU) y = gelu_tanh_fast2(y);
-      const int64_t o = (int64_t)orow[r] * e.ldo + n;
-      if (MODE == EPI_RESID) {
-        const float2 res = ldg2(e.resid + o);
-        const float2 gt = per_row_gate ? ldg2(e.gate + (int64_t)mrow[r] * e.gate_ld + n) : g0;
-        y.x = fmaf(gt.x, y.x, res.x); y.y = fmaf(gt.y, y.y, res.y);
+    for (int h = 0; h < 2; ++h) {
+      const int n = c0 + 32 * (2 * q + h);
+      if (rw.valid[r] && n < N) prefetch_l2(e.resid + (int64_t)rw.orow[r] * e.ldo + n);
+    }
+  }
+}
+
+// Epilogue of one consumer thread's accumulators: rows rw.orow, column pairs col0 + 8 j (j < 32).  Every access of a quad of
+// lanes covers 32 contiguous bytes of a row.  MODE / GELU are compile-time so that the per-element path carries no mode
+// branches.  The columns go in batches of CH pairs: every load of a batch (bias, gate, residual, addtab) is issued before its
+// first store.  The output may alias the residual (the in-place residual stream), so a load placed after a store could not be
+// moved ahead of it and each pair would pay a full global round trip.  Per element the arithmetic is unchanged.
+template <int MODE, bool GELU>
+__device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&acc)[ACC], const EpiRows& rw, int col0, int N) {
+  constexpr int CH = MODE == EPI_RESID ? 4 : 8;        // residual + gate of both rows: 8 registers per pair
+  const bool per_row_gate = MODE == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
+  const bool per_row_add = MODE == EPI_STORE && e.addtab;
+  const bool fp16 = e.fp16 != 0;
+  const float2 zero = make_float2(0.f, 0.f), one = make_float2(1.f, 1.f);
+#pragma unroll
+  for (int c = 0; c < BN / 8; c += CH) {
+    float2 bias[CH], res[2][CH], gt[2][CH], add[2][CH];
+#pragma unroll
+    for (int i = 0; i < CH; ++i) {
+      const int n = col0 + 8 * (c + i);
+      const bool in = n < N;                             // N % 4 == 0 and n even: a pair is all in or all out
+      bias[i] = e.bias && in ? ldg2(e.bias + n) : zero;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const bool v = in && rw.valid[r];
+        const int64_t o = (int64_t)rw.orow[r] * e.ldo + n;
+        if (MODE == EPI_RESID) {
+          res[r][i] = v ? ldg2(e.resid + o) : zero;
+          gt[r][i] = v && e.gate ? ldg2(per_row_gate ? e.gate + (int64_t)rw.mrow[r] * e.gate_ld + n : e.gate + n) : one;
+        }
+        if (MODE == EPI_STORE) add[r][i] = v && per_row_add ? ldg2(e.addtab + (int64_t)rw.mrow[r] * e.add_ld + n) : zero;
       }
-      if (MODE == EPI_SPLIT) {
-        const uint32_t hi = pack2_sat16(y.x, y.y, fp16);
-        *reinterpret_cast<uint32_t*>(e.out_hi + o) = hi;
-        if (e.out_lo) {                                  // bf16x3: residual planes
-          const float lx = y.x - __bfloat162float(__float2bfloat16_rn(y.x)), ly = y.y - __bfloat162float(__float2bfloat16_rn(y.y));
-          *reinterpret_cast<uint32_t*>(e.out_lo + o) = pack2_sat16(lx, ly, false);
+    }
+#pragma unroll
+    for (int i = 0; i < CH; ++i) {
+      const int j = c + i;
+      const int n = col0 + 8 * j;
+      if (n >= N) continue;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        if (!rw.valid[r]) continue;
+        float2 y = make_float2(acc[4 * j + 2 * r] + bias[i].x, acc[4 * j + 2 * r + 1] + bias[i].y);
+        if (GELU) y = gelu_tanh_fast2(y);
+        const int64_t o = (int64_t)rw.orow[r] * e.ldo + n;
+        if (MODE == EPI_RESID) {
+          y.x = fmaf(gt[r][i].x, y.x, res[r][i].x); y.y = fmaf(gt[r][i].y, y.y, res[r][i].y);
         }
-      } else {
-        if (per_row_add) {
-          const float2 a = ldg2(e.addtab + (int64_t)mrow[r] * e.add_ld + n);
-          y.x += a.x; y.y += a.y;
+        if (MODE == EPI_SPLIT) {
+          const uint32_t hi = pack2_sat16(y.x, y.y, fp16);
+          *reinterpret_cast<uint32_t*>(e.out_hi + o) = hi;
+          if (e.out_lo) {                                // bf16x3: residual planes
+            const float lx = y.x - __bfloat162float(__float2bfloat16_rn(y.x)), ly = y.y - __bfloat162float(__float2bfloat16_rn(y.y));
+            *reinterpret_cast<uint32_t*>(e.out_lo + o) = pack2_sat16(lx, ly, false);
+          }
+        } else {
+          if (per_row_add) { y.x += add[r][i].x; y.y += add[r][i].y; }
+          *reinterpret_cast<float2*>(e.out + o) = y;
         }
-        *reinterpret_cast<float2*>(e.out + o) = y;
       }
     }
   }
 }
 
 // mode / activation dispatch (uniform across the grid)
-__device__ __forceinline__ void epilogue_dispatch(const Epilogue& e, const float (&acc)[ACC], int64_t row0, int64_t M, int col0, int N) {
-  if (e.mode == EPI_RESID) epilogue_tile<EPI_RESID, false>(e, acc, row0, M, col0, N);
+__device__ __forceinline__ void epilogue_dispatch(const Epilogue& e, const float (&acc)[ACC], const EpiRows& rw, int col0, int N) {
+  if (e.mode == EPI_RESID) epilogue_tile<EPI_RESID, false>(e, acc, rw, col0, N);
   else if (e.mode == EPI_SPLIT) {
-    if (e.act == ACT_GELU) epilogue_tile<EPI_SPLIT, true>(e, acc, row0, M, col0, N);
-    else epilogue_tile<EPI_SPLIT, false>(e, acc, row0, M, col0, N);
+    if (e.act == ACT_GELU) epilogue_tile<EPI_SPLIT, true>(e, acc, rw, col0, N);
+    else epilogue_tile<EPI_SPLIT, false>(e, acc, rw, col0, N);
   } else {
-    if (e.act == ACT_GELU) epilogue_tile<EPI_STORE, true>(e, acc, row0, M, col0, N);
-    else epilogue_tile<EPI_STORE, false>(e, acc, row0, M, col0, N);
+    if (e.act == ACT_GELU) epilogue_tile<EPI_STORE, true>(e, acc, rw, col0, N);
+    else epilogue_tile<EPI_STORE, false>(e, acc, rw, col0, N);
   }
 }
 
@@ -194,6 +246,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
 
   if (warp >= CONSUMERS * 4) {
     // =========================================================== TMA producer
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == CONSUMERS * 4 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       // The weight tile is re-read by every group of M tiles; without a hint the activation / residual / output streams of the
@@ -247,6 +300,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
     }
   } else {
     // =========================================================== consumer warpgroups: wgmma + epilogue
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2;                                        // rows [64 wg, 64 wg + 64) of the CTA's 128
     const bool signaller = (threadIdx.x & 127) == 0;
     auto release = [&](int s) {                                      // the stage's wgmma reads have completed
@@ -261,6 +315,12 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
       if (second) tile_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
       else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
       const int nk = ((second ? p1.K : p0.K) + BK - 1) / BK;
+      const int wl = threadIdx.x & 127;
+      const int64_t row0 = (int64_t)(pm * CL + (int)rank) * BM + wg * 64 + (wl >> 5) * 16 + ((wl & 31) >> 2);
+      const int col0 = n_blk * BN + 2 * (wl & 3);
+      // the two problems are handled by separate (statically addressed) copies of the epilogue
+      const EpiRows rw = second ? epilogue_rows(p1.ep, row0, p1.M) : epilogue_rows(p0.ep, row0, p0.M);
+      const int pf_kb = nk > kPrefetchKBlocks ? nk - kPrefetchKBlocks : 0;
       float acc[ACC];
 #pragma unroll
       for (int i = 0; i < ACC; ++i) acc[i] = 0.f;
@@ -284,6 +344,10 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
           }
         }
         wgmma_commit();
+        if (kb == pf_kb) {
+          if (!second) epilogue_prefetch(p0.ep, rw, col0, p0.N);
+          else epilogue_prefetch(p1.ep, rw, col0, p1.N);
+        }
         wgmma_wait<1>();                                             // the previous stage's MMAs have retired
         if (prev >= 0) release(prev);
         prev = stage;
@@ -292,12 +356,8 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
       wgmma_wait<0>();
       fence_regs(acc);
       release(prev);
-      const int wl = threadIdx.x & 127;
-      const int64_t row0 = (int64_t)(pm * CL + (int)rank) * BM + wg * 64 + (wl >> 5) * 16 + ((wl & 31) >> 2);
-      const int col0 = n_blk * BN + 2 * (wl & 3);
-      // the two problems are handled by separate (statically addressed) copies of the epilogue
-      if (!second) epilogue_dispatch(p0.ep, acc, row0, p0.M, col0, p0.N);
-      else epilogue_dispatch(p1.ep, acc, row0, p1.M, col0, p1.N);
+      if (!second) epilogue_dispatch(p0.ep, acc, rw, col0, p0.N);
+      else epilogue_dispatch(p1.ep, acc, rw, col0, p1.N);
     }
   }
   // ---- teardown: nobody may exit while a peer can still multicast into its shared memory or arrive on its barriers

@@ -83,6 +83,15 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   return pol;
 }
 
+// warpgroup-wide register reallocation (every thread of the warpgroup executes it)
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// fetch the 128 B line holding `p` into L2 (a hint: no register result, nothing waits on it)
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<uint64_t>(p)));
+}
+
 // ---------------------------------------------------------------------------------------------- cluster
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
