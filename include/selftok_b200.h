@@ -239,13 +239,53 @@ int selftok_set_profile(selftok_handle_t h, int enable);
 int selftok_get_profile(selftok_handle_t h, double* ms_out /*[8]*/, int64_t* count_out /*[8]*/);
 
 /* ---- kernel-level entry points (parity tests and micro-benchmarks call these through the same ABI) ---------- */
-/* y[M,N] = act(A[M,K] W[N,K]^T + bias) (+ epilogue), fp32 FFMA.  act: 0 none, 1 gelu-tanh, 2 silu. */
-int selftok_k_linear_f32(const float* A_dev, const float* W_dev, const float* bias_dev, float* out_dev,
-                         int64_t M, int N, int K, int act, void* stream);
-/* Same product on the tensor-core (wgmma) path: A/W given as fp32, converted to 16-bit planes internally
- * (nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass). */
-int selftok_k_linear_tc(const float* A_dev, const float* W_dev, const float* bias_dev, float* out_dev,
-                        int64_t M, int N, int K, int nsplit, void* stream);
+/* GEMM epilogue, field for field the one both GEMM kernels implement.  y = act(A W^T + bias) of GEMM row m, then
+ *   mode 0 (store)    : out[orow, n] = y (+ addtab[trow * add_ld + n])
+ *   mode 1 (residual) : out[orow, n] = resid[orow, n] + gate[trow * gate_ld + n] * y   (gate NULL -> 1; out may alias resid)
+ *   mode 2 (split)    : out_hi / out_lo[orow, n] = bf16 hi / lo split of y (fp16 != 0: out_hi = IEEE half of y saturated to
+ *                       +-65504, NaN kept, and out_lo must be NULL)
+ * trow = tab_rows[m] if given, else m % add_period (store) or m % gate_period (residual).
+ * orow = row_map[m] if given; else with a token-range plan ([B][2] int32 (a_b, c_b)) the slot row of the plan (plan_ctx 1:
+ * context stream, rpb_in = Kc; 0: image stream, rpb_in = image rows, row_off = Kc); else (m / rpb_in) * rpb_out + row_off +
+ * m % rpb_in when rpb_in > 0; else m.  act: 0 none, 1 GELU-tanh, 2 SiLU (fp32 FFMA path only).  All pointers are device
+ * pointers; fp32 bases must be 8-byte and 16-bit plane bases 4-byte aligned.  ldo is in elements of the output. */
+typedef struct selftok_k_epilogue {
+  int32_t mode, act;
+  const float* bias;
+  float* out;
+  int64_t ldo;
+  const float* resid;
+  const float* gate;
+  int64_t gate_ld;
+  int32_t gate_period;
+  const float* addtab;
+  int64_t add_ld;
+  int32_t add_period;
+  void* out_hi;                /* 16-bit planes (bf16 or IEEE half bits) */
+  void* out_lo;
+  int32_t rpb_in, rpb_out, row_off;
+  int32_t fp16;
+  const int32_t* plan;
+  int32_t plan_ctx;
+  const int32_t* tab_rows;     /* [M] */
+  const int32_t* row_map;      /* [M] */
+} selftok_k_epilogue_t;
+/* One GEMM: fp32 device A [M, K] and W [N, K], row-major.  conv_C > 0 (tensor-core path): implicit 3x3 convolution, padding 1,
+ * K = 9 conv_C with K index (ky * 3 + kx) * conv_C + c; A is NHWC [M / (conv_H conv_W), conv_H, conv_W, conv_C] for
+ * conv_stride 1, and for conv_stride 2 the four polyphase planes of the input [images * 4 + py * 2 + px, conv_H, conv_W, conv_C]
+ * (plane[y][x] = in[2y + py][2x + px], zero padding right / bottom), conv_H / conv_W being the output dims. */
+typedef struct selftok_k_gemm_problem {
+  const float* A;
+  const float* W;
+  int64_t M;
+  int32_t N, K;
+  int32_t conv_C, conv_H, conv_W, conv_stride;
+  selftok_k_epilogue_t ep;
+} selftok_k_gemm_problem_t;
+/* path 0: fp32 FFMA kernel, one problem, no convolution (nsplit ignored).  path 1: wgmma kernel, one or two problems in one
+ * launch; A / W are converted to 16-bit planes first (nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass).
+ * Returns after the work has finished.  Epilogue errors are reported before anything runs on the device. */
+int selftok_k_gemm(int path, int nsplit, const selftok_k_gemm_problem_t* problems, int n, void* stream);
 /* Process-wide choice of the GEMM variant: 2 = two-CTA clusters sharing the weight tile by TMA multicast (default),
  * 1 = one CTA per tile. */
 int selftok_k_set_gemm_ctas(int n);

@@ -25,7 +25,7 @@ SYMBOLS = [
     "selftok_set_schedule", "selftok_finalize", "selftok_export_packed", "selftok_import_packed", "selftok_encode", "selftok_vq_argmax", "selftok_lookup",
     "selftok_set_cfg_schedule", "selftok_decode", "selftok_decode_cfg", "selftok_dit_velocity", "selftok_render", "selftok_encode_host", "selftok_decode_host",
     "selftok_render_host", "selftok_id_errors", "selftok_workspace_bytes", "selftok_set_workspace", "selftok_last_launch_count", "selftok_device_bytes", "selftok_set_use_graph",
-    "selftok_set_profile", "selftok_get_profile", "selftok_k_linear_f32", "selftok_k_linear_tc", "selftok_k_set_gemm_ctas", "selftok_k_ln_mod_f32", "selftok_k_attention_f32",
+    "selftok_set_profile", "selftok_get_profile", "selftok_k_gemm", "selftok_k_set_gemm_ctas", "selftok_k_ln_mod_f32", "selftok_k_attention_f32",
     "selftok_k_attention_tc", "selftok_decode_range", "selftok_decode_cfg_range", "selftok_render_range", "selftok_k_attention_tc_range",
     "selftok_decode_step",
     "selftok_vae_create", "selftok_vae_destroy", "selftok_vae_load_tensor", "selftok_vae_finalize", "selftok_vae_decode", "selftok_vae_encode", "selftok_vae_device_bytes",
@@ -41,6 +41,23 @@ class _Config(C.Structure):
         "K", "latent", "in_channels", "enc_patch", "enc_hidden", "enc_heads", "enc_depth", "enc_qdim", "enc_qheads",
         "enc_pos_max", "codebook_size", "code_dim", "dit_depth", "dit_patch", "dit_pos_max", "renderer",
         "context_see_xt", "precision", "device")]
+
+
+class KEpilogue(C.Structure):
+    """selftok_k_epilogue_t (include/selftok_b200.h): pointers are device addresses (int), 0 for NULL."""
+    _fields_ = [("mode", C.c_int32), ("act", C.c_int32), ("bias", C.c_void_p), ("out", C.c_void_p), ("ldo", C.c_int64),
+                ("resid", C.c_void_p), ("gate", C.c_void_p), ("gate_ld", C.c_int64), ("gate_period", C.c_int32),
+                ("addtab", C.c_void_p), ("add_ld", C.c_int64), ("add_period", C.c_int32),
+                ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("rpb_in", C.c_int32), ("rpb_out", C.c_int32), ("row_off", C.c_int32), ("fp16", C.c_int32),
+                ("plan", C.c_void_p), ("plan_ctx", C.c_int32), ("tab_rows", C.c_void_p), ("row_map", C.c_void_p)]
+
+
+class KGemmProblem(C.Structure):
+    """selftok_k_gemm_problem_t."""
+    _fields_ = [("A", C.c_void_p), ("W", C.c_void_p), ("M", C.c_int64), ("N", C.c_int32), ("K", C.c_int32),
+                ("conv_C", C.c_int32), ("conv_H", C.c_int32), ("conv_W", C.c_int32), ("conv_stride", C.c_int32),
+                ("ep", KEpilogue)]
 
 
 _lib = None
@@ -89,8 +106,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.selftok_set_use_graph.argtypes = [vp, i32]
     lib.selftok_set_profile.argtypes = [vp, i32]
     lib.selftok_get_profile.argtypes = [vp, vp, vp]
-    lib.selftok_k_linear_f32.argtypes = [vp, vp, vp, vp, i64, i32, i32, i32, vp]
-    lib.selftok_k_linear_tc.argtypes = [vp, vp, vp, vp, i64, i32, i32, i32, vp]
+    lib.selftok_k_gemm.argtypes = [i32, i32, C.POINTER(KGemmProblem), i32, vp]
     lib.selftok_k_set_gemm_ctas.argtypes = [i32]
     lib.selftok_k_ln_mod_f32.argtypes = [vp, vp, vp, i64, i32, vp, i64, i32, vp]
     lib.selftok_k_attention_f32.argtypes = [vp, i64, vp, vp, i64, i32, vp, vp, i64, i32, vp, i64, i32, i32, i32, i32, vp]
@@ -635,21 +651,58 @@ class VaeDecoder:
 
 
 # ---- kernel-level helpers used by tests and micro-benchmarks ---------------------------------------------------
+_EPI_MODES = {"store": 0, "resid": 1, "split": 2}
+_EPI_ACTS = {"none": 0, "gelu": 1, "silu": 2}
+
+
+def _addr(v) -> int:
+    """Device address of a tensor (its data_ptr, views included) or a raw int; None -> NULL."""
+    if v is None:
+        return 0
+    return v.data_ptr() if isinstance(v, torch.Tensor) else int(v)
+
+
+def k_gemm_problem(A, W, M, N, K, *, conv=None, mode="store", act="none", **ep) -> KGemmProblem:
+    """One selftok_k_gemm_problem_t.  A, W and every pointer field of `ep` (bias, out, resid, gate, addtab, out_hi, out_lo,
+    plan, tab_rows, row_map) take a tensor or a raw address; the integer fields (ldo, gate_ld, gate_period, add_ld, add_period,
+    rpb_in, rpb_out, row_off, fp16, plan_ctx) take ints.  conv = (C, H, W, stride) selects the implicit 3x3 convolution."""
+    ptrs = ("bias", "out", "resid", "gate", "addtab", "out_hi", "out_lo", "plan", "tab_rows", "row_map")
+    e = KEpilogue(mode=_EPI_MODES.get(mode, mode), act=_EPI_ACTS.get(act, act), gate_period=1, add_period=1)
+    for k, v in ep.items():
+        if k not in dict(KEpilogue._fields_):
+            raise TypeError(f"unknown epilogue field {k!r}")
+        setattr(e, k, _addr(v) if k in ptrs else int(v))
+    q = KGemmProblem(A=_addr(A), W=_addr(W), M=M, N=N, K=K, ep=e)
+    if conv is not None:
+        q.conv_C, q.conv_H, q.conv_W, q.conv_stride = conv
+    return q
+
+
+def k_gemm_status(path: int, nsplit: int, problems, stream=None) -> int:
+    """selftok_k_gemm on one or two problems (path 0: fp32 FFMA, 1: wgmma); returns the raw status.  Synchronous."""
+    arr = (KGemmProblem * len(problems))(*problems)
+    if stream is None:
+        stream = torch.cuda.current_stream().cuda_stream if torch.cuda.is_available() else 0
+    return load_library().selftok_k_gemm(path, nsplit, arr, len(problems), stream)
+
+
+def k_gemm(path: int, nsplit: int, problems, stream=None) -> None:
+    check(k_gemm_status(path, nsplit, problems, stream))
+
+
 def k_linear_f32(A, W, bias=None, act=0):
-    lib = load_library()
     M, K = A.shape
     N = W.shape[0]
     out = torch.empty(M, N, dtype=torch.float32, device=A.device)
-    check(lib.selftok_k_linear_f32(A.data_ptr(), W.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K, act, _stream_ptr(A.device)))
+    k_gemm(0, 3, [k_gemm_problem(A, W, M, N, K, act=act, bias=bias, out=out, ldo=N)], _stream_ptr(A.device))
     return out
 
 
 def k_linear_tc(A, W, bias=None, nsplit=3):
-    lib = load_library()
     M, K = A.shape
     N = W.shape[0]
     out = torch.empty(M, N, dtype=torch.float32, device=A.device)
-    check(lib.selftok_k_linear_tc(A.data_ptr(), W.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K, nsplit, _stream_ptr(A.device)))
+    k_gemm(1, nsplit, [k_gemm_problem(A, W, M, N, K, bias=bias, out=out, ldo=N)], _stream_ptr(A.device))
     return out
 
 

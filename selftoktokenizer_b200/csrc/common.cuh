@@ -94,26 +94,28 @@ __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bflo
 __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
   return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
+// two fp32 -> one packed 16-bit pair (lo in bits 0-15): IEEE half with saturation to +-65504 (one F2FP.SATFINITE instead of
+// two clamps + convert; +-inf saturates too, NaN stays NaN), or bf16 round-to-nearest
+__device__ __forceinline__ uint32_t pack2_sat16(float lo, float hi, bool fp16) {
+  uint32_t r;
+  if (fp16) asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  else asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
 // 16-bit operand planes hold either bf16 (hi [+ lo] split) or, in the single-pass fp16 mode, IEEE half values; the
-// storage type is __nv_bfloat16 in both cases (the bits are what the tensor core is told they are).
+// storage type is __nv_bfloat16 in both cases (the bits are what the tensor core is told they are).  The half conversion is
+// the one the tensor-core epilogues use (pack2_sat16), so a value converts to the same bits on every path: a clamp with
+// fminf / fmaxf would turn NaN into -65504.
 __device__ __forceinline__ void split16(float x, bool fp16, uint16_t& hi, uint16_t& lo) {
   if (fp16) {
-    hi = __half_as_ushort(__float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f)));   // saturate instead of overflowing to inf
+    hi = (uint16_t)(pack2_sat16(x, 0.f, true) & 0xffffu);
     lo = 0;
   } else {
     __nv_bfloat16 h = __float2bfloat16_rn(x);
     hi = __bfloat16_as_ushort(h);
     lo = __bfloat16_as_ushort(__float2bfloat16_rn(x - __bfloat162float(h)));
   }
-}
-
-// two fp32 -> one packed 16-bit pair (lo in bits 0-15): IEEE half with saturation to +-65504 (one F2FP.SATFINITE instead of
-// two clamps + convert), or bf16 round-to-nearest
-__device__ __forceinline__ uint32_t pack2_sat16(float lo, float hi, bool fp16) {
-  uint32_t r;
-  if (fp16) asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  else asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
 }
 // bf16 residual plane of a pair: lo = rn(x - rn_bf16(x))
 __device__ __forceinline__ uint32_t pack2_resid_bf16(float a, float b, uint32_t hi_pair) {

@@ -1665,36 +1665,75 @@ extern "C" __attribute__((visibility("default"))) int64_t selftok_last_launch_co
 extern "C" __attribute__((visibility("default"))) int64_t selftok_device_bytes(selftok_handle_t e) { return e ? e->bytes : -1; }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI
-extern "C" __attribute__((visibility("default"))) int selftok_k_linear_f32(const float* A, const float* W, const float* bias, float* out, int64_t M, int N, int K,
-                                    int act, void* stream) {
+static Epilogue k_epilogue(const selftok_k_epilogue_t& d) {
   Epilogue ep;
-  ep.act = act; ep.bias = bias; ep.out = out; ep.ldo = N;
-  return launch_linear_f32(A, K, W, K, M, N, K, ep, (cudaStream_t)stream);
+  ep.mode = d.mode; ep.act = d.act; ep.bias = d.bias; ep.out = d.out; ep.ldo = d.ldo;
+  ep.resid = d.resid; ep.gate = d.gate; ep.gate_ld = d.gate_ld; ep.gate_period = d.gate_period;
+  ep.addtab = d.addtab; ep.add_ld = d.add_ld; ep.add_period = d.add_period;
+  ep.out_hi = (bf16*)d.out_hi; ep.out_lo = (bf16*)d.out_lo;
+  ep.rpb_in = d.rpb_in; ep.rpb_out = d.rpb_out; ep.row_off = d.row_off; ep.fp16 = d.fp16;
+  ep.plan = d.plan; ep.plan_ctx = d.plan_ctx; ep.tab_rows = d.tab_rows; ep.row_map = d.row_map;
+  return ep;
 }
 
-extern "C" __attribute__((visibility("default"))) int selftok_k_linear_tc(const float* A, const float* W, const float* bias, float* out, int64_t M, int N, int K,
-                                   int ns, void* stream) {
-  STK_CHECK(A && W && out && (ns == 0 || ns == 1 || ns == 3), SELFTOK_ERR_BAD_ARG, "selftok_k_linear_tc: bad argument");
-  const int fp16 = ns == 0;
-  if (fp16) ns = 1;
-  STK_TRY(gemm_tc_init());
-  cudaStream_t s = (cudaStream_t)stream;
-  bf16 *ah, *al = nullptr, *wh, *wl = nullptr;
-  STK_CUDA(cudaMalloc(&ah, sizeof(bf16) * M * K));
-  STK_CUDA(cudaMalloc(&wh, sizeof(bf16) * (int64_t)N * K));
-  if (ns == 3) {
-    STK_CUDA(cudaMalloc(&al, sizeof(bf16) * M * K));
-    STK_CUDA(cudaMalloc(&wl, sizeof(bf16) * (int64_t)N * K));
+// fp32 elements of a problem's A operand in the layout the kernel reads (stride-2 convolutions: four polyphase planes per image)
+static int64_t k_gemm_a_elems(const selftok_k_gemm_problem_t& q) {
+  if (q.conv_C <= 0) return q.M * q.K;
+  return q.M * q.conv_C * (q.conv_stride == 2 ? 4 : 1);
+}
+
+extern "C" __attribute__((visibility("default"))) int selftok_k_gemm(int path, int ns, const selftok_k_gemm_problem_t* probs, int n, void* stream) {
+  STK_CHECK(probs && (path == 0 || path == 1) && n >= 1 && n <= (path == 0 ? 1 : 2), SELFTOK_ERR_BAD_ARG,
+            "selftok_k_gemm: path 0 takes one problem, path 1 one or two");
+  STK_CHECK(path == 0 || ns == 0 || ns == 1 || ns == 3, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: nsplit must be 3, 1 or 0");
+  Epilogue eps[2];
+  for (int i = 0; i < n; ++i) {
+    const selftok_k_gemm_problem_t& q = probs[i];
+    STK_CHECK(q.A && q.W && q.M > 0 && q.N > 0 && q.K > 0, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: bad operands or shape");
+    STK_CHECK(path == 1 || q.conv_C == 0, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: the fp32 FFMA path has no convolution mode");
+    eps[i] = k_epilogue(q.ep);
+    STK_TRY(check_epilogue(eps[i], "selftok_k_gemm"));   // before any CUDA call
   }
-  int st = launch_split_bf16(A, ah, al, M * K, s, fp16);
-  if (!st) st = launch_split_bf16(W, wh, wl, (int64_t)N * K, s, fp16);
-  Epilogue ep;
-  ep.bias = bias; ep.out = out; ep.ldo = N;
-  if (!st) st = launch_gemm_tc(ah, al, wh, wl, M, N, K, ns, ep, s, fp16);
-  cudaStreamSynchronize(s);
-  cudaFree(ah); cudaFree(wh);
-  if (al) cudaFree(al);
-  if (wl) cudaFree(wl);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (path == 0) {
+    const selftok_k_gemm_problem_t& q = probs[0];
+    STK_TRY(launch_linear_f32(q.A, q.K, q.W, q.K, q.M, q.N, q.K, eps[0], s));
+    STK_CUDA(cudaStreamSynchronize(s));
+    return SELFTOK_OK;
+  }
+  const int fp16 = ns == 0;
+  const int nsplit = ns == 3 ? 3 : 1;
+  STK_TRY(gemm_tc_init());
+  bf16* planes[2][4] = {};                                // per problem: A hi, A lo, W hi, W lo
+  TcProblem tp[2];
+  int st = 0;
+  for (int i = 0; i < n && !st; ++i) {
+    const selftok_k_gemm_problem_t& q = probs[i];
+    const int64_t na = k_gemm_a_elems(q), nw = (int64_t)q.N * q.K;
+    for (int p = 0; p < 4 && !st; ++p) {
+      if ((p & 1) && nsplit != 3) continue;
+      if (cudaMalloc(&planes[i][p], sizeof(bf16) * (p < 2 ? na : nw)) != cudaSuccess) {
+        set_error("selftok_k_gemm: cudaMalloc of the operand planes failed");
+        st = SELFTOK_ERR_CUDA;
+      }
+    }
+    if (st) break;
+    tp[i] = TcProblem{planes[i][0], planes[i][1], planes[i][2], planes[i][3], q.M, q.N, q.K, eps[i]};
+    tp[i].conv_C = q.conv_C; tp[i].conv_H = q.conv_H; tp[i].conv_W = q.conv_W; tp[i].conv_stride = q.conv_stride;
+    st = check_gemm_tc_problem(tp[i], nsplit, fp16);      // shape / geometry errors before any launch
+  }
+  for (int i = 0; i < n && !st; ++i) {
+    st = launch_split_bf16(probs[i].A, planes[i][0], planes[i][1], k_gemm_a_elems(probs[i]), s, fp16);
+    if (!st) st = launch_split_bf16(probs[i].W, planes[i][2], planes[i][3], (int64_t)probs[i].N * probs[i].K, s, fp16);
+  }
+  if (!st) st = launch_gemm_tc_grouped(tp, n, nsplit, s, fp16);
+  if (cudaStreamSynchronize(s) != cudaSuccess && !st) {
+    set_error("selftok_k_gemm: the stream failed");
+    st = SELFTOK_ERR_CUDA;
+  }
+  for (auto& pl : planes)
+    for (bf16* p : pl)
+      if (p) cudaFree(p);
   return st;
 }
 

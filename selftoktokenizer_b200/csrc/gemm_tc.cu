@@ -462,11 +462,15 @@ int gemm_tc_init() {
   return 0;
 }
 
-static int check_problem(const TcProblem& q, int nsplit, int fp16) {
+int check_gemm_tc_problem(const TcProblem& q, int nsplit, int fp16) {
   const Epilogue& ep = q.ep;
   STK_CHECK(q.A_hi && q.W_hi && q.M > 0 && q.N > 0 && q.K > 0, -1, "gemm_tc: bad arguments");
   STK_CHECK(nsplit == 1 || (nsplit == 3 && q.A_lo && q.W_lo), -1, "gemm_tc: nsplit must be 1, or 3 with lo planes");
   STK_CHECK(!fp16 || nsplit == 1, -1, "gemm_tc: the fp16 mode is single-pass");
+  auto aligned16 = [](const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; };
+  STK_CHECK(aligned16(q.A_hi) && aligned16(q.A_lo) && aligned16(q.W_hi) && aligned16(q.W_lo), -1,
+            "gemm_tc: operand planes must be 16-byte aligned (TMA)");
+  STK_TRY(check_epilogue(ep, "gemm_tc"));
   STK_CHECK(ep.act == ACT_NONE || (ep.act == ACT_GELU && ep.mode != EPI_RESID), -2,
             "gemm_tc: epilogue activation must be none, or GELU-tanh with the store / split modes");
   STK_CHECK(ep.mode != EPI_STORE || ep.addtab == nullptr || ep.add_ld % 4 == 0, -2, "gemm_tc: addtab pitch must be a multiple of 4");
@@ -533,7 +537,7 @@ int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream
   int dev = 0;
   STK_CUDA(cudaGetDevice(&dev));
   const int g_num_sms = g_num_sms_dev[dev];
-  for (int i = 0; i < n; ++i) STK_TRY(check_problem(probs[i], nsplit, fp16));
+  for (int i = 0; i < n; ++i) STK_TRY(check_gemm_tc_problem(probs[i], nsplit, fp16));
   const int CL = g_gemm_ctas == 2 && g_num_sms >= 2 ? 2 : 1;
   TcMaps m0, m1;
   STK_TRY(make_maps(&m0, probs[0], nsplit, fp16, BN / CL));

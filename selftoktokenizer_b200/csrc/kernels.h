@@ -32,7 +32,7 @@ struct Epilogue {
   int64_t add_ld = 0;
   int add_period = 1;
   __nv_bfloat16* out_hi = nullptr;       // EPI_SPLIT
-  __nv_bfloat16* out_lo = nullptr;       // may be NULL (single-pass bf16)
+  __nv_bfloat16* out_lo = nullptr;       // may be NULL (single-pass bf16); must be NULL with fp16
   int rpb_in = 0, rpb_out = 0, row_off = 0;
   int fp16 = 0;                          // EPI_SPLIT: planes hold IEEE half (single-pass fp16 mode) instead of bf16
   const int* plan = nullptr;             // token-range plan of this step, [B][2] int32 (a, c); NULL: plain remap
@@ -45,6 +45,10 @@ __host__ __device__ __forceinline__ int plan_slot_row(int r, int a, int c, int n
   if (!ctx) return c + r;
   return r < a ? c + n_img + r : (r < a + c ? r - a : n_img + r);
 }
+// Host-side checks of an epilogue that both GEMM launchers make before any launch (SELFTOK_ERR_BAD_ARG on failure): the
+// pointers its mode needs are set, periods are >= 1, the fp32 bases (bias, out, resid, gate, addtab) are 8-byte aligned and
+// the 16-bit plane bases 4-byte aligned (the wgmma epilogue moves column pairs), and the fp16 split mode has no out_lo plane.
+int check_epilogue(const Epilogue& ep, const char* who);
 
 // ---- fp32 FFMA kernels (kernels_simt.cu) ---------------------------------------------------------------------
 int launch_linear_f32(const float* A, int64_t lda, const float* W, int64_t ldw, int64_t M, int N, int K,
@@ -157,6 +161,8 @@ struct TcProblem {
 };
 // one launch for one or two independent problems of the same operand type
 int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream_t s, int fp16 = 0);
+// the host-side checks launch_gemm_tc_grouped makes of each problem (no CUDA call)
+int check_gemm_tc_problem(const TcProblem& q, int nsplit, int fp16);
 int gemm_tc_init();   // resolves cuTensorMapEncodeTiled, sets smem attributes; idempotent
 void gemm_tc_set_ctas(int n);   // 2 (default): two-CTA clusters sharing the W tile by TMA multicast; 1: one CTA per tile
 

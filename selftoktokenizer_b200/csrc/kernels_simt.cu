@@ -153,12 +153,28 @@ __global__ void __launch_bounds__(256, 2) linear_f32_kernel(const LinParams p) {
   }
 }
 
+int check_epilogue(const Epilogue& ep, const char* who) {
+  const std::string w(who);
+  auto aligned = [](const void* p, uintptr_t a) { return reinterpret_cast<uintptr_t>(p) % a == 0; };
+  STK_CHECK(ep.mode == EPI_STORE || ep.mode == EPI_RESID || ep.mode == EPI_SPLIT, -1, w + ": unknown epilogue mode");
+  STK_CHECK(ep.mode != EPI_SPLIT ? ep.out != nullptr : ep.out_hi != nullptr, -1, w + ": the epilogue has no output");
+  STK_CHECK(ep.mode != EPI_RESID || ep.resid != nullptr, -1, w + ": the residual mode needs resid");
+  STK_CHECK(ep.gate_period >= 1 && ep.add_period >= 1, -1, w + ": table periods must be >= 1");
+  STK_CHECK(!ep.plan || ep.row_map || ep.rpb_in > 0, -1, w + ": a token-range plan needs rpb_in > 0");
+  STK_CHECK(aligned(ep.bias, 8) && aligned(ep.out, 8) && aligned(ep.resid, 8) && aligned(ep.gate, 8) && aligned(ep.addtab, 8), -1,
+            w + ": bias, out, resid, gate and addtab must be 8-byte aligned");
+  STK_CHECK(aligned(ep.out_hi, 4) && aligned(ep.out_lo, 4), -1, w + ": 16-bit output planes must be 4-byte aligned");
+  STK_CHECK(!(ep.fp16 && ep.out_lo), -1, w + ": the fp16 split mode writes no lo plane (out_lo must be NULL)");
+  return 0;
+}
+
 int launch_linear_f32(const float* A, int64_t lda, const float* W, int64_t ldw, int64_t M, int N, int K,
                       const Epilogue& ep, cudaStream_t s) {
   STK_CHECK(A && W && M > 0 && N > 0 && K > 0, -1, "linear_f32: bad arguments");
   STK_CHECK(K % 4 == 0 && lda % 4 == 0 && ldw % 4 == 0, -2, "linear_f32: K and leading dims must be multiples of 4");
   STK_CHECK((reinterpret_cast<uintptr_t>(A) % 16 == 0) && (reinterpret_cast<uintptr_t>(W) % 16 == 0), -1,
             "linear_f32: operands must be 16-byte aligned");
+  STK_TRY(check_epilogue(ep, "linear_f32"));
   LinParams p{A, lda, W, ldw, M, N, K, ep};
   if (N > 64 && M > 64) {
     dim3 grid((N + 127) / 128, (unsigned)((M + 127) / 128));

@@ -44,6 +44,49 @@ def test_sass_contains_hopper_tensor_and_tma_instructions():
     assert not re.search(r"\bHMMA", sass), "legacy mma.sync instructions found in the library"
 
 
+_BASE = 1 << 40          # a 256-byte aligned address; the calls below are rejected before any CUDA call, so nothing is read
+
+
+def _k_gemm_case(name):
+    M, N, K = 64, 64, 64
+    a = lambda i: _BASE + i * (1 << 24)
+    store = dict(mode="store", out=a(3), ldo=N, bias=a(4))
+    resid = dict(mode="resid", out=a(3), ldo=N, resid=a(5), gate=a(6), gate_ld=N)
+    split = dict(mode="split", out_hi=a(7), out_lo=a(8), ldo=N)
+    ep = {"bias": dict(store, bias=a(4) + 4), "out": dict(store, out=a(3) + 4), "addtab": dict(store, addtab=a(9) + 4, add_ld=N),
+          "resid": dict(resid, resid=a(5) + 4), "gate": dict(resid, gate=a(6) + 4), "in_place_out": dict(resid, out=a(5) + 4, resid=a(5) + 4),
+          "out_hi": dict(split, out_hi=a(7) + 2), "out_lo": dict(split, out_lo=a(8) + 2), "fp16_out_lo": dict(split, fp16=1),
+          "no_out": dict(store, out=0), "no_resid": dict(resid, resid=0), "no_plane": dict(split, out_hi=0),
+          "mode": dict(store, mode=3), "gate_period": dict(resid, gate_period=0), "plan_without_rpb": dict(store, plan=a(10))}[name]
+    return capi.k_gemm_problem(a(1), a(2), M, N, K, **ep)
+
+
+@pytest.mark.parametrize("path,nsplit", [(0, 3), (1, 3), (1, 1), (1, 0)])
+@pytest.mark.parametrize("case", ["bias", "out", "addtab", "resid", "gate", "in_place_out", "out_hi", "out_lo", "fp16_out_lo",
+                                  "no_out", "no_resid", "no_plane", "mode", "gate_period", "plan_without_rpb"])
+def test_k_gemm_rejects_bad_epilogue_before_any_cuda_call(case, path, nsplit):
+    """Misaligned fp32 bases (the wgmma epilogue moves float2 pairs) and 16-bit plane bases (32-bit pairs), an out_lo plane in the
+    fp16 split mode, missing outputs and bad periods are SELFTOK_ERR_BAD_ARG from both GEMM paths, found on the host: the
+    addresses here point at nothing, so a call that got as far as the device would fail differently."""
+    B.build()
+    st = capi.k_gemm_status(path, nsplit, [_k_gemm_case(case)], stream=0)
+    assert st == -1, (st, capi.load_library().selftok_last_error())
+    assert b"selftok_k_gemm" in capi.load_library().selftok_last_error()
+
+
+def test_k_gemm_rejects_bad_calls():
+    B.build()
+    q = _k_gemm_case("bias")
+    q.ep.bias = _BASE
+    assert capi.k_gemm_status(0, 3, [q, q], stream=0) == -1        # the FFMA path takes one problem
+    assert capi.k_gemm_status(1, 2, [q], stream=0) == -1           # nsplit 3 / 1 / 0
+    assert capi.k_gemm_status(2, 3, [q], stream=0) == -1
+    q.conv_C, q.conv_H, q.conv_W, q.conv_stride = 64, 8, 8, 1
+    assert capi.k_gemm_status(0, 3, [q], stream=0) == -1           # no convolution on the FFMA path
+    q.conv_C, q.M = 0, 0
+    assert capi.k_gemm_status(1, 3, [q], stream=0) == -1
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU behaviour")
 def test_no_cpu_fallback():
     B.build()
