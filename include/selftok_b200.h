@@ -60,7 +60,12 @@ typedef enum selftok_precision {
   SELFTOK_PREC_FP32_SIMT = 0,     /* fp32 FFMA GEMMs + fp32 attention (bring-up / bisecting reference)       */
   SELFTOK_PREC_BF16X3 = 1,        /* wgmma: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, fp32 accumulate             */
   SELFTOK_PREC_BF16 = 2,          /* wgmma single pass (bf16 operands, fp32 accumulate)                    */
-  SELFTOK_PREC_FP16 = 3           /* wgmma single pass (IEEE half operands, fp32 accumulate)               */
+  SELFTOK_PREC_FP16 = 3,          /* wgmma single pass (IEEE half operands, fp32 accumulate)               */
+  SELFTOK_PREC_FP8 = 4            /* SELFTOK_PREC_FP16, except that the QKV and fc1 GEMMs of both streams (the two whose A operand
+                                   * is LayerNorm + modulate) run on e4m3 operands: activations with one fp32 scale per row,
+                                   * weights with one per output channel, scale = amax / 448, fp32 accumulate, both scales
+                                   * applied in the epilogue.  proj, fc2, attention, the patch embedding and the final layer
+                                   * stay as in fp16; the encoder, VQ and VAE are not affected.                           */
 } selftok_precision;
 
 /* Flat view of cfg.tokenizer.params (configs/res256/256-eval.yml:48-105) after the reference's registries
@@ -283,7 +288,9 @@ typedef struct selftok_k_gemm_problem {
   selftok_k_epilogue_t ep;
 } selftok_k_gemm_problem_t;
 /* path 0: fp32 FFMA kernel, one problem, no convolution (nsplit ignored).  path 1: wgmma kernel, one or two problems in one
- * launch; A / W are converted to 16-bit planes first (nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass).
+ * launch; A / W are converted to 16-bit planes first (nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass), or, with
+ * nsplit 4, quantized to e4m3 per row (A per GEMM row, W per output channel; selftok_k_quant_e4m3), no convolution; the epilogue
+ * then sees y = fma(acc, s_a[m] * s_w[n], bias) with m the GEMM row before any remap.
  * Returns after the work has finished.  Epilogue errors are reported before anything runs on the device. */
 int selftok_k_gemm(int path, int nsplit, const selftok_k_gemm_problem_t* problems, int n, void* stream);
 /* Process-wide choice of the GEMM variant: 2 = two-CTA clusters sharing the weight tile by TMA multicast (default),
@@ -292,6 +299,14 @@ int selftok_k_set_gemm_ctas(int n);
 /* out = LN(x) * (1 + scale[m % period]) + shift[m % period], rows of D; eps 1e-6, no affine. */
 int selftok_k_ln_mod_f32(const float* x_dev, const float* shift_dev, const float* scale_dev, int64_t ld_mod,
                          int period, float* out_dev, int64_t M, int D, void* stream);
+/* e4m3 quantization of fp32 rows x [M, K] (K % 4 == 0): scale_m = amax_m / 448 and codes cvt.rn.satfinite.e4m3(x * (448 / amax_m))
+ * (both quotients correctly rounded), codes_out [M, K] bytes, scales_out [M] fp32.  amax is NaN for a row holding a NaN; an
+ * all-zero row gives scale 0 and zero codes; a non-finite amax is not sanitised. */
+int selftok_k_quant_e4m3(const float* x_dev, int64_t M, int K, void* codes_out_dev, float* scales_out_dev, void* stream);
+/* The fp8 decoder's LayerNorm + modulate (as selftok_k_ln_mod_f32, shift / scale required; period > 1 needs M % period == 0)
+ * with the e4m3 output of the same rule: codes_out [M, D] bytes, scales_out [M] fp32.  D % 16 == 0. */
+int selftok_k_ln_mod_e4m3(const float* x_dev, const float* shift_dev, const float* scale_dev, int64_t ld_mod, int period,
+                          void* codes_out_dev, float* scales_out_dev, int64_t M, int D, void* stream);
 /* softmax(Q K^T / sqrt(hd)) V, fp32; q [B,Sq,H*hd], k/v two concatenated segments [B,S1,H*hd] + [B,S2,H*hd]
  * (S2 may be 0), each with its own row stride in floats. */
 int selftok_k_attention_f32(const float* q_dev, int64_t q_ld, const float* k1_dev, const float* v1_dev, int64_t kv1_ld,

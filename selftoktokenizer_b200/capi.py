@@ -17,7 +17,8 @@ from . import schedule as sched
 from .config import SelftokDims
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc", "libselftok_b200.so")
-PREC = {"fp32": 0, "bf16x3": 1, "bf16": 2, "fp16": 3}
+# "fp8": the fp16 mode with e4m3 QKV and fc1 GEMMs (per-row activation and per-channel weight scales); never chosen by "auto"
+PREC = {"fp32": 0, "bf16x3": 1, "bf16": 2, "fp16": 3, "fp8": 4}
 
 # every symbol include/selftok_b200.h declares (tests check the .so exports exactly these)
 SYMBOLS = [
@@ -27,7 +28,7 @@ SYMBOLS = [
     "selftok_render_host", "selftok_id_errors", "selftok_workspace_bytes", "selftok_set_workspace", "selftok_last_launch_count", "selftok_device_bytes", "selftok_set_use_graph",
     "selftok_set_profile", "selftok_get_profile", "selftok_k_gemm", "selftok_k_set_gemm_ctas", "selftok_k_ln_mod_f32", "selftok_k_attention_f32",
     "selftok_k_attention_tc", "selftok_decode_range", "selftok_decode_cfg_range", "selftok_render_range", "selftok_k_attention_tc_range",
-    "selftok_decode_step",
+    "selftok_decode_step", "selftok_k_quant_e4m3", "selftok_k_ln_mod_e4m3",
     "selftok_vae_create", "selftok_vae_destroy", "selftok_vae_load_tensor", "selftok_vae_finalize", "selftok_vae_decode", "selftok_vae_encode", "selftok_vae_device_bytes",
 ]
 
@@ -109,6 +110,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.selftok_k_gemm.argtypes = [i32, i32, C.POINTER(KGemmProblem), i32, vp]
     lib.selftok_k_set_gemm_ctas.argtypes = [i32]
     lib.selftok_k_ln_mod_f32.argtypes = [vp, vp, vp, i64, i32, vp, i64, i32, vp]
+    lib.selftok_k_quant_e4m3.argtypes = [vp, i64, i32, vp, vp, vp]
+    lib.selftok_k_ln_mod_e4m3.argtypes = [vp, vp, vp, i64, i32, vp, vp, i64, i32, vp]
     lib.selftok_k_attention_f32.argtypes = [vp, i64, vp, vp, i64, i32, vp, vp, i64, i32, vp, i64, i32, i32, i32, i32, vp]
     lib.selftok_k_attention_tc.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.selftok_decode_range.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp]
@@ -717,6 +720,25 @@ def k_ln_mod_f32(x, shift=None, scale=None, period=1):
     ld = shift.shape[-1] if shift is not None else 0
     check(lib.selftok_k_ln_mod_f32(x.data_ptr(), _ptr(shift), _ptr(scale), ld, period, out.data_ptr(), M, D, _stream_ptr(x.device)))
     return out
+
+
+def k_quant_e4m3(x):
+    """fp32 rows x [M, K] -> (codes [M, K] torch.float8_e4m3fn, scales [M] fp32): scale = amax / 448 per row (include/selftok_b200.h)."""
+    M, K = x.shape
+    codes = torch.empty(M, K, dtype=torch.uint8, device=x.device)
+    scales = torch.empty(M, dtype=torch.float32, device=x.device)
+    check(load_library().selftok_k_quant_e4m3(x.data_ptr(), M, K, codes.data_ptr(), scales.data_ptr(), _stream_ptr(x.device)))
+    return codes.view(torch.float8_e4m3fn), scales
+
+
+def k_ln_mod_e4m3(x, shift, scale, period=1):
+    """LN + modulate of x [M, D] as k_ln_mod_f32, quantized to e4m3 with one scale per row -> (codes [M, D], scales [M])."""
+    M, D = x.shape
+    codes = torch.empty(M, D, dtype=torch.uint8, device=x.device)
+    scales = torch.empty(M, dtype=torch.float32, device=x.device)
+    check(load_library().selftok_k_ln_mod_e4m3(x.data_ptr(), shift.data_ptr(), scale.data_ptr(), shift.shape[-1], period,
+                                               codes.data_ptr(), scales.data_ptr(), M, D, _stream_ptr(x.device)))
+    return codes.view(torch.float8_e4m3fn), scales
 
 
 def k_attention_f32(q, k1, v1, k2=None, v2=None, heads=1):

@@ -125,6 +125,32 @@ __device__ __forceinline__ uint32_t pack2_resid_bf16(float a, float b, uint32_t 
   return r;
 }
 
+// ---- e4m3 quantization (the contract in kernels.h) ----
+// max that keeps NaN (fmaxf drops it)
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float warp_max_nan(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+// row amax -> (inv, scale): inv = 448 / amax, scale = amax / 448, both 0 for an all-zero row
+__device__ __forceinline__ void e4m3_row_scale(float amax, float& inv, float& scale) {
+  inv = amax == 0.f ? 0.f : __fdiv_rn(448.f, amax);
+  scale = __fdiv_rn(amax, 448.f);
+}
+// four fp32 -> four e4m3 codes (x0 in the low byte): cvt.rn.satfinite of x_i * inv
+__device__ __forceinline__ uint32_t pack4_e4m3(float x0, float x1, float x2, float x3, float inv) {
+  const float a = __fmul_rn(x0, inv), b = __fmul_rn(x1, inv), c = __fmul_rn(x2, inv), d = __fmul_rn(x3, inv);
+  uint16_t lo, hi;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
+  return (uint32_t)lo | ((uint32_t)hi << 16);
+}
+
 // element pairs: (d0, d1) = (a0, a1) * (b0, b1) + (c0, c1) and (d0, d1) = (a0, a1) + (b0, b1), each lane rounded once
 __device__ __forceinline__ void ffma2(float a0, float a1, float b0, float b1, float c0, float c1, float& d0, float& d1) {
   d0 = __fmaf_rn(a0, b0, c0);

@@ -32,8 +32,9 @@ struct Tensor {
   int64_t numel = 0;
 };
 struct WPack {
-  bf16* hi = nullptr;
+  bf16* hi = nullptr;                   // fp8 mode, qkv / fc1: e4m3 codes [N, K] (one byte each)
   bf16* lo = nullptr;
+  float* scale = nullptr;               // fp8 mode, qkv / fc1: [N] per-output-channel scales of the codes
 };
 
 // Bump allocator over ONE block of device memory: the activation workspaces are carved from it.  The block is either the
@@ -69,6 +70,7 @@ struct DecodeWs {       // activation workspace of the MMDiT for one batch size
   bf16 *a_c_hi = nullptr, *a_c_lo = nullptr, *a_x_hi = nullptr, *a_x_lo = nullptr;
   bf16 *attn_c_hi = nullptr, *attn_c_lo = nullptr, *attn_x_hi = nullptr, *attn_x_lo = nullptr;
   bf16 *h_c_hi = nullptr, *h_c_lo = nullptr, *h_x_hi = nullptr, *h_x_lo = nullptr;
+  float *sa_c = nullptr, *sa_x = nullptr;        // fp8 mode: row scales of the e4m3 codes in a_c_hi / a_x_hi
   int* plan = nullptr;                           // token-range calls: [B][2] windows (lo, hi), then the plan [steps][B][2] (a, c)
   int* pk = nullptr;                             // step calls: the per-image block (see Packed), then the per-row maps
   void* own = nullptr;                           // the library's own block (NULL when the caller's workspace is in use)
@@ -171,7 +173,13 @@ static const Tensor* find(selftok_engine* e, const std::string& name) {
 
 static bool tc_mode(const selftok_engine* e) { return e->cfg.precision != SELFTOK_PREC_FP32_SIMT; }
 static int nsplit(const selftok_engine* e) { return e->cfg.precision == SELFTOK_PREC_BF16X3 ? 3 : 1; }
-static int is_fp16(const selftok_engine* e) { return e->cfg.precision == SELFTOK_PREC_FP16 ? 1 : 0; }
+// the fp8 mode is the fp16 mode with e4m3 QKV and fc1 GEMMs: every 16-bit plane of it holds IEEE half
+static int is_fp16(const selftok_engine* e) { return e->cfg.precision == SELFTOK_PREC_FP16 || e->cfg.precision == SELFTOK_PREC_FP8 ? 1 : 0; }
+static bool is_fp8(const selftok_engine* e) { return e->cfg.precision == SELFTOK_PREC_FP8; }
+// the linears that run on e4m3 operands in the fp8 mode: the two whose A operand comes from LayerNorm + modulate
+static bool e4m3_linear(const std::string& name) {
+  return name.find(".attn.qkv.") != std::string::npos || name.find(".mlp.fc1.") != std::string::npos;
+}
 
 // y = act(A W^T + b) with weights looked up by checkpoint prefix (fp32 FFMA path)
 static int lin32(selftok_engine* e, const std::string& prefix, const float* A, int64_t lda, int64_t M, Epilogue ep,
@@ -201,9 +209,10 @@ static int lintc(selftok_engine* e, const std::string& prefix, const bf16* A_hi,
   return 0;
 }
 
-// tensor-core problem descriptor for a checkpoint linear (weights already packed at finalize)
+// tensor-core problem descriptor for a checkpoint linear (weights already packed at finalize).  e4m3-packed weights (fp8 mode):
+// A_hi holds e4m3 codes and s_a their row scales.
 static int tc_problem(selftok_engine* e, const std::string& prefix, const bf16* A_hi, const bf16* A_lo, int64_t M, Epilogue ep,
-                      TcProblem* out) {
+                      TcProblem* out, const float* s_a = nullptr) {
   GETW(W, prefix + ".weight");
   GETW(Bv, prefix + ".bias");
   auto it = e->wp.find(prefix + ".weight");
@@ -213,12 +222,17 @@ static int tc_problem(selftok_engine* e, const std::string& prefix, const bf16* 
   ep.bias = Bv->d;
   if (ep.ldo == 0) ep.ldo = N;
   ep.fp16 = is_fp16(e);
+  if (it->second.scale) {
+    STK_CHECK(s_a, SELFTOK_ERR_STATE, "e4m3 weights need the row scales of A");
+    ep.s_a = s_a; ep.s_w = it->second.scale;
+  }
   *out = TcProblem{A_hi, A_lo, it->second.hi, it->second.lo, M, N, K, ep};
   return 0;
 }
-// the context- and image-stream GEMM of a layer in ONE launch (n == 1: image stream only)
-static int lintc2(selftok_engine* e, const TcProblem* probs, int n, cudaStream_t s) {
-  PROF(PC_GEMM_TC, launch_gemm_tc_grouped(probs, n, nsplit(e), s, is_fp16(e)));
+// the context- and image-stream GEMM of a layer in ONE launch (n == 1: image stream only); e4m3: the fp8 mode's QKV / fc1
+static int lintc2(selftok_engine* e, const TcProblem* probs, int n, cudaStream_t s, bool e4m3 = false) {
+  if (e4m3) PROF(PC_GEMM_TC, launch_gemm_tc_grouped(probs, n, NSPLIT_E4M3, s, 0));
+  else PROF(PC_GEMM_TC, launch_gemm_tc_grouped(probs, n, nsplit(e), s, is_fp16(e)));
   return 0;
 }
 
@@ -247,7 +261,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_create(const selft
   int hd1 = cfg->enc_hidden / cfg->enc_heads, hd2 = cfg->enc_qdim / cfg->enc_qheads;
   STK_CHECK((hd1 == 16 || hd1 == 32 || hd1 == 64) && (hd2 == 16 || hd2 == 32 || hd2 == 64), SELFTOK_ERR_UNSUPPORTED,
             "encoder head_dim must be 16/32/64");
-  STK_CHECK(cfg->precision >= 0 && cfg->precision <= 3, SELFTOK_ERR_BAD_ARG, "bad precision");
+  STK_CHECK(cfg->precision >= 0 && cfg->precision <= SELFTOK_PREC_FP8, SELFTOK_ERR_BAD_ARG, "bad precision");
   STK_CUDA(cudaSetDevice(cfg->device));
   selftok_engine* e = new selftok_engine();
   e->cfg = *cfg;
@@ -469,6 +483,17 @@ extern "C" __attribute__((visibility("default"))) int selftok_finalize(selftok_h
           std::string name = "model.joint_blocks." + std::to_string(j) + "." + blocks[b] + "." + lins[l] + ".weight";
           GETW(W, name);
           WPack p;
+          if (is_fp8(e) && e4m3_linear(name)) {                 // e4m3 codes + one scale per output channel
+            const int64_t N = W->shape[0];
+            uint8_t* codes;
+            STK_TRY(dalloc(e, e->allocs, &codes, W->numel));
+            STK_TRY(dalloc(e, e->allocs, &p.scale, N));
+            PROF(PC_OTHER, launch_quant_e4m3_rows(W->d, N, (int)(W->numel / N), codes, p.scale, s));
+            p.hi = reinterpret_cast<bf16*>(codes);
+            e->wp[name] = p;
+            packed_names.push_back(name);
+            continue;
+          }
           STK_TRY(dalloc(e, e->allocs, &p.hi, W->numel));
           if (nsplit(e) == 3) STK_TRY(dalloc(e, e->allocs, &p.lo, W->numel));
           PROF(PC_OTHER, launch_split_bf16(W->d, p.hi, p.lo, W->numel, s, is_fp16(e)));
@@ -586,9 +611,14 @@ extern "C" __attribute__((visibility("default"))) int selftok_export_packed(self
   for (auto& kv : e->wp) {
     if (!ok) break;
     const int64_t numel = e->w[kv.first].numel;
-    const uint32_t has_lo = kv.second.lo != nullptr;
-    ok = io.wstr(kv.first) && io.w(&numel, 8) && io.w(&has_lo, 4) && io.wdev(kv.second.hi, 2 * (size_t)numel);
-    if (ok && has_lo) ok = io.wdev(kv.second.lo, 2 * (size_t)numel);
+    // kind 0: one 16-bit plane, 1: hi + lo planes, 2: e4m3 codes (1 byte each) + [N] fp32 scales
+    const uint32_t kind = kv.second.scale ? 2u : kv.second.lo != nullptr ? 1u : 0u;
+    ok = io.wstr(kv.first) && io.w(&numel, 8) && io.w(&kind, 4) && io.wdev(kv.second.hi, (kind == 2 ? 1 : 2) * (size_t)numel);
+    if (ok && kind == 1) ok = io.wdev(kv.second.lo, 2 * (size_t)numel);
+    if (ok && kind == 2) {
+      const int64_t n = e->w[kv.first].shape[0];
+      ok = io.w(&n, 8) && io.wdev(kv.second.scale, sizeof(float) * (size_t)n);
+    }
   }
   for (const TableRef& t : table_refs(e)) {
     if (!ok) break;
@@ -645,12 +675,20 @@ extern "C" __attribute__((visibility("default"))) int selftok_import_packed(self
   for (uint32_t i = 0; ok && i < n_p; ++i) {
     std::string name;
     int64_t numel = 0;
-    uint32_t has_lo = 0;
+    uint32_t kind = 0;
     WPack pk;
-    ok = io.rstr(name) && io.r(&numel, 8) && io.r(&has_lo, 4) && numel > 0;
+    ok = io.rstr(name) && io.r(&numel, 8) && io.r(&kind, 4) && numel > 0 && kind <= 2;
     if (!ok) break;
-    ok = dalloc(e, e->allocs, &pk.hi, numel) == 0 && io.rdev(pk.hi, 2 * (size_t)numel);
-    if (ok && has_lo) ok = dalloc(e, e->allocs, &pk.lo, numel) == 0 && io.rdev(pk.lo, 2 * (size_t)numel);
+    if (kind == 2) {                                          // e4m3 codes + per-channel scales
+      uint8_t* codes = nullptr;
+      int64_t n = 0;
+      ok = dalloc(e, e->allocs, &codes, numel) == 0 && io.rdev(codes, (size_t)numel) && io.r(&n, 8) && n > 0 && numel % n == 0 &&
+           dalloc(e, e->allocs, &pk.scale, n) == 0 && io.rdev(pk.scale, sizeof(float) * (size_t)n);
+      pk.hi = reinterpret_cast<bf16*>(codes);
+    } else {
+      ok = dalloc(e, e->allocs, &pk.hi, numel) == 0 && io.rdev(pk.hi, 2 * (size_t)numel);
+      if (ok && kind == 1) ok = dalloc(e, e->allocs, &pk.lo, numel) == 0 && io.rdev(pk.lo, 2 * (size_t)numel);
+    }
     e->wp[name] = pk;
   }
   for (const TableRef& t : table_refs(e)) {
@@ -943,6 +981,10 @@ static int layout_dws(selftok_engine* e, DecodeWs& w, int64_t B, Arena& A) {
     STK_TRY(A.take(&w.attn_x_hi, B * N * D));
     STK_TRY(A.take(&w.h_c_hi, B * K * 4 * D));
     STK_TRY(A.take(&w.h_x_hi, B * N * 4 * D));
+    if (is_fp8(e)) {                                          // row scales of the e4m3 LN outputs (QKV / fc1 A operands)
+      STK_TRY(A.take(&w.sa_c, B * K));
+      STK_TRY(A.take(&w.sa_x, B * N));
+    }
     if (lo) {
       STK_TRY(A.take(&w.a_c_lo, B * K * D));
       STK_TRY(A.take(&w.a_x_lo, B * N * D));
@@ -1094,6 +1136,9 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
     if (tc_mode(e)) {
       // ---- tensor-core path: the two streams' GEMMs of every stage share one launch (lintc2)
       const int fp16 = is_fp16(e);
+      // fp8 mode: the LN launches write e4m3 codes + row scales into a_*_hi, and the QKV / fc1 GEMMs run on e4m3
+      const bool fp8 = is_fp8(e);
+      const int ln16 = fp8 ? 0 : fp16;
       const float* lm = e->ctx_last_mod + (int64_t)step * 2 * D;                // last layer: pre_only (shift, scale) from c
       // LN + modulate of both streams in one launch (context rows: per-position adaLN table; image rows: the step's row)
       LnProblem lp[2];
@@ -1102,17 +1147,18 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       else { lp[0].shift = lm; lp[0].scale = lm + D; lp[0].ld_mod = 2 * D; lp[0].period = 1; lp[0].rows = rows_cl; }
       lp[1].x = w.x; lp[1].out_hi = w.a_x_hi; lp[1].out_lo = w.a_x_lo; lp[1].M = Mx;
       lp[1].shift = xmod; lp[1].scale = xmod + D; lp[1].ld_mod = 6 * D; lp[1].period = 1; lp[1].rows = rows_x;
-      if (ctx) PROF(PC_LN, launch_ln_mod_pair(lp, 2, D, 1e-6f, s, fp16));
-      else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, fp16));
+      if (fp8) { lp[0].out_scale = w.sa_c; lp[1].out_scale = w.sa_x; }
+      if (ctx) PROF(PC_LN, launch_ln_mod_pair(lp, 2, D, 1e-6f, s, ln16));
+      else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, ln16));
       TcProblem pr[2];
       Epilogue eq;                                                              // q/k/v leave the GEMM as 16-bit planes in the joint buffer
       eq.mode = EPI_SPLIT; eq.out_hi = w.qkv_hi; eq.out_lo = w.qkv_lo; eq.ldo = 3 * D; eq.rpb_out = S; eq.plan = plan;
       int np = 0;
       eq.rpb_in = Kc; eq.row_off = 0; eq.plan_ctx = 1; eq.row_map = map_c;
-      if (ctx) STK_TRY(tc_problem(e, pc + "attn.qkv", w.a_c_hi, w.a_c_lo, Mc, eq, &pr[np++]));
+      if (ctx) STK_TRY(tc_problem(e, pc + "attn.qkv", w.a_c_hi, w.a_c_lo, Mc, eq, &pr[np++], w.sa_c));
       eq.rpb_in = N; eq.row_off = Kc; eq.plan_ctx = 0; eq.row_map = nullptr;
-      STK_TRY(tc_problem(e, px + "attn.qkv", w.a_x_hi, w.a_x_lo, Mx, eq, &pr[np++]));
-      STK_TRY(lintc2(e, pr, np, s));
+      STK_TRY(tc_problem(e, px + "attn.qkv", w.a_x_hi, w.a_x_lo, Mx, eq, &pr[np++], w.sa_x));
+      STK_TRY(lintc2(e, pr, np, s, fp8));
       AttnOut ao;
       ao.split = Kc; ao.ld = D;
       ao.hi_a = w.attn_c_hi; ao.lo_a = w.attn_c_lo; ao.hi_b = w.attn_x_hi; ao.lo_b = w.attn_x_lo;
@@ -1130,15 +1176,15 @@ static int joint_blocks(selftok_engine* e, int B, int Kc, int step, bool ctx_sel
       STK_TRY(lintc2(e, pr, np, s));
       lp[0].shift = cmod + 3 * D; lp[0].scale = cmod + 4 * D; lp[0].ld_mod = 6 * D; lp[0].period = Kc; lp[0].rows = rows_c;
       lp[1].shift = xmod + 3 * D; lp[1].scale = xmod + 4 * D;
-      if (ctx_post) PROF(PC_LN, launch_ln_mod_pair(lp, 2, D, 1e-6f, s, fp16));
-      else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, fp16));
+      if (ctx_post) PROF(PC_LN, launch_ln_mod_pair(lp, 2, D, 1e-6f, s, ln16));
+      else PROF(PC_LN, launch_ln_mod_pair(lp + 1, 1, D, 1e-6f, s, ln16));
       Epilogue ehc, ehx;
       ehc.mode = EPI_SPLIT; ehc.act = ACT_GELU; ehc.out_hi = w.h_c_hi; ehc.out_lo = w.h_c_lo; ehc.ldo = 4 * D;
       ehx = ehc; ehx.out_hi = w.h_x_hi; ehx.out_lo = w.h_x_lo;
       np = 0;
-      if (ctx_post) STK_TRY(tc_problem(e, pc + "mlp.fc1", w.a_c_hi, w.a_c_lo, Mc, ehc, &pr[np++]));
-      STK_TRY(tc_problem(e, px + "mlp.fc1", w.a_x_hi, w.a_x_lo, Mx, ehx, &pr[np++]));
-      STK_TRY(lintc2(e, pr, np, s));
+      if (ctx_post) STK_TRY(tc_problem(e, pc + "mlp.fc1", w.a_c_hi, w.a_c_lo, Mc, ehc, &pr[np++], w.sa_c));
+      STK_TRY(tc_problem(e, px + "mlp.fc1", w.a_x_hi, w.a_x_lo, Mx, ehx, &pr[np++], w.sa_x));
+      STK_TRY(lintc2(e, pr, np, s, fp8));
       erc.gate = cmod + 5 * D; erx.gate = xmod + 5 * D;
       np = 0;
       if (ctx_post) STK_TRY(tc_problem(e, pc + "mlp.fc2", w.h_c_hi, w.h_c_lo, Mc, erc, &pr[np++]));
@@ -1685,12 +1731,14 @@ static int64_t k_gemm_a_elems(const selftok_k_gemm_problem_t& q) {
 extern "C" __attribute__((visibility("default"))) int selftok_k_gemm(int path, int ns, const selftok_k_gemm_problem_t* probs, int n, void* stream) {
   STK_CHECK(probs && (path == 0 || path == 1) && n >= 1 && n <= (path == 0 ? 1 : 2), SELFTOK_ERR_BAD_ARG,
             "selftok_k_gemm: path 0 takes one problem, path 1 one or two");
-  STK_CHECK(path == 0 || ns == 0 || ns == 1 || ns == 3, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: nsplit must be 3, 1 or 0");
+  STK_CHECK(path == 0 || ns == 0 || ns == 1 || ns == 3 || ns == NSPLIT_E4M3, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: nsplit must be 4, 3, 1 or 0");
+  const bool e4m3 = path == 1 && ns == NSPLIT_E4M3;
   Epilogue eps[2];
   for (int i = 0; i < n; ++i) {
     const selftok_k_gemm_problem_t& q = probs[i];
     STK_CHECK(q.A && q.W && q.M > 0 && q.N > 0 && q.K > 0, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: bad operands or shape");
     STK_CHECK(path == 1 || q.conv_C == 0, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: the fp32 FFMA path has no convolution mode");
+    STK_CHECK(!e4m3 || q.conv_C == 0, SELFTOK_ERR_BAD_ARG, "selftok_k_gemm: the e4m3 mode has no convolution");
     eps[i] = k_epilogue(q.ep);
     STK_TRY(check_epilogue(eps[i], "selftok_k_gemm"));   // before any CUDA call
   }
@@ -1702,27 +1750,43 @@ extern "C" __attribute__((visibility("default"))) int selftok_k_gemm(int path, i
     return SELFTOK_OK;
   }
   const int fp16 = ns == 0;
-  const int nsplit = ns == 3 ? 3 : 1;
+  const int nsplit = e4m3 ? NSPLIT_E4M3 : ns == 3 ? 3 : 1;
   STK_TRY(gemm_tc_init());
-  bf16* planes[2][4] = {};                                // per problem: A hi, A lo, W hi, W lo
+  bf16* planes[2][4] = {};                                // per problem: A hi, A lo, W hi, W lo (e4m3: A codes, A scales, W codes, W scales)
   TcProblem tp[2];
   int st = 0;
   for (int i = 0; i < n && !st; ++i) {
     const selftok_k_gemm_problem_t& q = probs[i];
     const int64_t na = k_gemm_a_elems(q), nw = (int64_t)q.N * q.K;
     for (int p = 0; p < 4 && !st; ++p) {
-      if ((p & 1) && nsplit != 3) continue;
-      if (cudaMalloc(&planes[i][p], sizeof(bf16) * (p < 2 ? na : nw)) != cudaSuccess) {
+      if ((p & 1) && nsplit != 3 && !e4m3) continue;
+      // e4m3: one byte per code, one fp32 scale per row
+      const size_t bytes = e4m3 ? ((p & 1) ? sizeof(float) * (size_t)(p < 2 ? q.M : q.N) : (size_t)(p < 2 ? na : nw))
+                                : sizeof(bf16) * (size_t)(p < 2 ? na : nw);
+      if (cudaMalloc(&planes[i][p], bytes) != cudaSuccess) {
         set_error("selftok_k_gemm: cudaMalloc of the operand planes failed");
         st = SELFTOK_ERR_CUDA;
       }
     }
     if (st) break;
-    tp[i] = TcProblem{planes[i][0], planes[i][1], planes[i][2], planes[i][3], q.M, q.N, q.K, eps[i]};
+    if (e4m3) {
+      eps[i].s_a = reinterpret_cast<const float*>(planes[i][1]);
+      eps[i].s_w = reinterpret_cast<const float*>(planes[i][3]);
+      tp[i] = TcProblem{planes[i][0], nullptr, planes[i][2], nullptr, q.M, q.N, q.K, eps[i]};
+    } else {
+      tp[i] = TcProblem{planes[i][0], planes[i][1], planes[i][2], planes[i][3], q.M, q.N, q.K, eps[i]};
+    }
     tp[i].conv_C = q.conv_C; tp[i].conv_H = q.conv_H; tp[i].conv_W = q.conv_W; tp[i].conv_stride = q.conv_stride;
     st = check_gemm_tc_problem(tp[i], nsplit, fp16);      // shape / geometry errors before any launch
   }
   for (int i = 0; i < n && !st; ++i) {
+    if (e4m3) {                                           // A per GEMM row, W per output channel (kernels.h contract)
+      st = launch_quant_e4m3_rows(probs[i].A, probs[i].M, probs[i].K, reinterpret_cast<uint8_t*>(planes[i][0]),
+                                  reinterpret_cast<float*>(planes[i][1]), s);
+      if (!st) st = launch_quant_e4m3_rows(probs[i].W, probs[i].N, probs[i].K, reinterpret_cast<uint8_t*>(planes[i][2]),
+                                           reinterpret_cast<float*>(planes[i][3]), s);
+      continue;
+    }
     st = launch_split_bf16(probs[i].A, planes[i][0], planes[i][1], k_gemm_a_elems(probs[i]), s, fp16);
     if (!st) st = launch_split_bf16(probs[i].W, planes[i][2], planes[i][3], (int64_t)probs[i].N * probs[i].K, s, fp16);
   }
@@ -1746,6 +1810,21 @@ extern "C" __attribute__((visibility("default"))) int selftok_k_set_gemm_ctas(in
 extern "C" __attribute__((visibility("default"))) int selftok_k_ln_mod_f32(const float* x, const float* shift, const float* scale, int64_t ld_mod, int period,
                                     float* out, int64_t M, int D, void* stream) {
   return launch_ln_mod(x, D, shift, scale, ld_mod, period, out, nullptr, nullptr, D, M, D, 1e-6f, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int selftok_k_quant_e4m3(const float* x, int64_t M, int K, void* codes_out,
+                                                                          float* scales_out, void* stream) {
+  return launch_quant_e4m3_rows(x, M, K, static_cast<uint8_t*>(codes_out), scales_out, (cudaStream_t)stream);
+}
+
+// the fp8 decoder's LN + modulate -> e4m3 launch (launch_ln_mod_pair, one problem)
+extern "C" __attribute__((visibility("default"))) int selftok_k_ln_mod_e4m3(const float* x, const float* shift, const float* scale, int64_t ld_mod,
+                                                                           int period, void* codes_out, float* scales_out, int64_t M, int D,
+                                                                           void* stream) {
+  LnProblem lp;
+  lp.x = x; lp.shift = shift; lp.scale = scale; lp.ld_mod = ld_mod; lp.period = period;
+  lp.out_hi = static_cast<bf16*>(codes_out); lp.out_scale = scales_out; lp.M = M;
+  return launch_ln_mod_pair(&lp, 1, D, 1e-6f, (cudaStream_t)stream, 0);
 }
 
 extern "C" __attribute__((visibility("default"))) int selftok_k_attention_f32(const float* q, int64_t q_ld, const float* k1, const float* v1, int64_t kv1_ld, int S1,

@@ -2,6 +2,8 @@
 //
 //   operands   bf16 planes, K-major.  NSPLIT == 1: y = A_hi W_hi^T.  NSPLIT == 3 ("bf16x3", fp32-faithful to ~2^-17):
 //              y = A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T, all three products accumulated into the same registers.
+//              E4M3: e4m3 codes with per-row scales (kernels.h), wgmma m64n256k32; a k-block is 128 elements, so the tiles, TMA
+//              boxes and descriptors (128 B per K row) are byte for byte those of the 16-bit modes.
 //   tile       128 x 256 x 64 per pipeline stage per CTA; two consumer warpgroups, each wgmma m64n256k16 on its 64 rows
 //   staging    TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared memory ring, mbarrier full/empty pairs
 //   roles      warpgroups 0-1: wgmma + epilogue (registers -> HBM) | warpgroup 2: TMA producer (1 thread)
@@ -23,7 +25,8 @@ namespace {
 
 using namespace hop;
 
-constexpr int BM = 128, BN = 256, BK = 64, WK = 16;
+constexpr int BM = 128, BN = 256, BK = 64, WK = 16;   // BK, WK: 16-bit elements (128 B / 32 B of a K row)
+constexpr int BK8 = 128;                               // e4m3 elements per k-block (the same 128 B)
 constexpr int A_TILE_BYTES = BM * BK * 2;      // 16 KiB
 constexpr int B_TILE_BYTES = BN * BK * 2;      // 32 KiB
 constexpr int CONSUMERS = 2;                   // warpgroups of 64 rows
@@ -54,8 +57,10 @@ __device__ __forceinline__ float2 ldg2(const float* p) { return *reinterpret_cas
 struct EpiRows {
   int orow[2], mrow[2];
   bool valid[2];
+  float sa[2];                                         // e4m3: A row scales (GEMM rows, before any remap)
 };
 
+template <bool E4M3>
 __device__ __forceinline__ EpiRows epilogue_rows(const Epilogue& e, int64_t row0, int64_t M) {
   const bool per_row_gate = e.mode == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
   const bool per_row_add = e.mode == EPI_STORE && e.addtab;
@@ -77,6 +82,7 @@ __device__ __forceinline__ EpiRows epilogue_rows(const Epilogue& e, int64_t row0
     }
     if (e.tab_rows && rw.valid[r]) rw.mrow[r] = e.tab_rows[mi];
     else rw.mrow[r] = per_row_gate ? mi % e.gate_period : (per_row_add ? mi % e.add_period : 0);
+    rw.sa[r] = E4M3 && rw.valid[r] ? e.s_a[mi] : 0.f;
   }
   return rw;
 }
@@ -102,7 +108,8 @@ __device__ __forceinline__ void epilogue_prefetch(const Epilogue& e, const EpiRo
 // branches.  The columns go in batches of CH pairs: every load of a batch (bias, gate, residual, addtab) is issued before its
 // first store.  The output may alias the residual (the in-place residual stream), so a load placed after a store could not be
 // moved ahead of it and each pair would pay a full global round trip.  Per element the arithmetic is unchanged.
-template <int MODE, bool GELU>
+// E4M3: y = fma(acc, s_a[m] * s_w[n], bias); the W scales are loaded with the bias.
+template <int MODE, bool GELU, bool E4M3>
 __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&acc)[ACC], const EpiRows& rw, int col0, int N) {
   constexpr int CH = MODE == EPI_RESID ? 4 : 8;        // residual + gate of both rows: 8 registers per pair
   const bool per_row_gate = MODE == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
@@ -111,12 +118,13 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&a
   const float2 zero = make_float2(0.f, 0.f), one = make_float2(1.f, 1.f);
 #pragma unroll
   for (int c = 0; c < BN / 8; c += CH) {
-    float2 bias[CH], res[2][CH], gt[2][CH], add[2][CH];
+    float2 bias[CH], sw[CH], res[2][CH], gt[2][CH], add[2][CH];
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
       const int n = col0 + 8 * (c + i);
       const bool in = n < N;                             // N % 4 == 0 and n even: a pair is all in or all out
       bias[i] = e.bias && in ? ldg2(e.bias + n) : zero;
+      if (E4M3) sw[i] = in ? ldg2(e.s_w + n) : zero;
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const bool v = in && rw.valid[r];
@@ -136,7 +144,12 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&a
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         if (!rw.valid[r]) continue;
-        float2 y = make_float2(acc[4 * j + 2 * r] + bias[i].x, acc[4 * j + 2 * r + 1] + bias[i].y);
+        float2 y;
+        if (E4M3) {
+          y = make_float2(fmaf(acc[4 * j + 2 * r], rw.sa[r] * sw[i].x, bias[i].x), fmaf(acc[4 * j + 2 * r + 1], rw.sa[r] * sw[i].y, bias[i].y));
+        } else {
+          y = make_float2(acc[4 * j + 2 * r] + bias[i].x, acc[4 * j + 2 * r + 1] + bias[i].y);
+        }
         if (GELU) y = gelu_tanh_fast2(y);
         const int64_t o = (int64_t)rw.orow[r] * e.ldo + n;
         if (MODE == EPI_RESID) {
@@ -159,14 +172,15 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& e, const float (&a
 }
 
 // mode / activation dispatch (uniform across the grid)
+template <bool E4M3>
 __device__ __forceinline__ void epilogue_dispatch(const Epilogue& e, const float (&acc)[ACC], const EpiRows& rw, int col0, int N) {
-  if (e.mode == EPI_RESID) epilogue_tile<EPI_RESID, false>(e, acc, rw, col0, N);
+  if (e.mode == EPI_RESID) epilogue_tile<EPI_RESID, false, E4M3>(e, acc, rw, col0, N);
   else if (e.mode == EPI_SPLIT) {
-    if (e.act == ACT_GELU) epilogue_tile<EPI_SPLIT, true>(e, acc, rw, col0, N);
-    else epilogue_tile<EPI_SPLIT, false>(e, acc, rw, col0, N);
+    if (e.act == ACT_GELU) epilogue_tile<EPI_SPLIT, true, E4M3>(e, acc, rw, col0, N);
+    else epilogue_tile<EPI_SPLIT, false, E4M3>(e, acc, rw, col0, N);
   } else {
-    if (e.act == ACT_GELU) epilogue_tile<EPI_STORE, true>(e, acc, rw, col0, N);
-    else epilogue_tile<EPI_STORE, false>(e, acc, rw, col0, N);
+    if (e.act == ACT_GELU) epilogue_tile<EPI_STORE, true, E4M3>(e, acc, rw, col0, N);
+    else epilogue_tile<EPI_STORE, false, E4M3>(e, acc, rw, col0, N);
   }
 }
 
@@ -210,11 +224,13 @@ __device__ __forceinline__ void tile_coords(int t, int pm_tiles, int n_tiles, in
 //   full[s]    per CTA: its own A box plus both halves of the W tile (one from each CTA of the cluster) complete_tx on it
 //   empty[s]   per CTA: counts the two consumer warpgroups of EVERY CTA of the cluster, because the producer of this CTA
 //              writes its half of the W tile into all of them
-template <int NSPLIT, int CL, bool FP16>
+template <int NSPLIT, int CL, bool FP16, bool E4M3>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcMaps maps1, const GemmParams p0, const GemmParams p1) {
   static_assert(NSPLIT == 1 || !FP16, "the fp16 mode is single-pass");
+  static_assert(!E4M3 || (NSPLIT == 1 && !FP16), "the e4m3 mode is single-pass on its own operand type");
   using C = Cfg<NSPLIT>;
+  constexpr int KB = E4M3 ? BK8 : BK;                   // elements per k-block
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;           // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
@@ -259,7 +275,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
         int pm, n_blk;
         if (second) tile_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
         else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
-        const int nk = (pp.K + BK - 1) / BK;
+        const int nk = (pp.K + KB - 1) / KB;
         const int m_row = (pm * CL + (int)rank) * BM;               // this CTA's 128 A rows
         const int n_row = n_blk * BN + (int)rank * (BN / CL);       // this CTA's share of the W tile
         // convolution: the 128 rows are 128 / bw image rows of bw pixels starting at (cb, cy, cx)
@@ -284,14 +300,14 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
             tma_load_4d(sa, &mp.a_hi, fb, c0, x0, y0, n0);
             if (NSPLIT == 3) tma_load_4d(sa + A_TILE_BYTES, &mp.a_lo, fb, c0, x0, y0, n0);
           } else {
-            tma_load_2d(sa, &mp.a_hi, fb, kb * BK, m_row);
+            tma_load_2d(sa, &mp.a_hi, fb, kb * KB, m_row);
             if (NSPLIT == 3) tma_load_2d(sa + A_TILE_BYTES, &mp.a_lo, fb, kb * BK, m_row);
           }
           if (CL > 1) {
-            tma_load_2d_mc(sb, &mp.b_hi, fb, kb * BK, n_row, (uint16_t)((1u << CL) - 1), w_policy);
+            tma_load_2d_mc(sb, &mp.b_hi, fb, kb * KB, n_row, (uint16_t)((1u << CL) - 1), w_policy);
             if (NSPLIT == 3) tma_load_2d_mc(sb + B_TILE_BYTES, &mp.b_lo, fb, kb * BK, n_row, (uint16_t)((1u << CL) - 1), w_policy);
           } else {
-            tma_load_2d_hint(sb, &mp.b_hi, fb, kb * BK, n_row, w_policy);
+            tma_load_2d_hint(sb, &mp.b_hi, fb, kb * KB, n_row, w_policy);
             if (NSPLIT == 3) tma_load_2d_hint(sb + B_TILE_BYTES, &mp.b_lo, fb, kb * BK, n_row, w_policy);
           }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
@@ -314,12 +330,12 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
       int pm, n_blk;
       if (second) tile_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
       else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
-      const int nk = ((second ? p1.K : p0.K) + BK - 1) / BK;
+      const int nk = ((second ? p1.K : p0.K) + KB - 1) / KB;
       const int wl = threadIdx.x & 127;
       const int64_t row0 = (int64_t)(pm * CL + (int)rank) * BM + wg * 64 + (wl >> 5) * 16 + ((wl & 31) >> 2);
       const int col0 = n_blk * BN + 2 * (wl & 3);
       // the two problems are handled by separate (statically addressed) copies of the epilogue
-      const EpiRows rw = second ? epilogue_rows(p1.ep, row0, p1.M) : epilogue_rows(p0.ep, row0, p0.M);
+      const EpiRows rw = second ? epilogue_rows<E4M3>(p1.ep, row0, p1.M) : epilogue_rows<E4M3>(p0.ep, row0, p0.M);
       const int pf_kb = nk > kPrefetchKBlocks ? nk - kPrefetchKBlocks : 0;
       float acc[ACC];
 #pragma unroll
@@ -334,9 +350,10 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / WK; ++k) {
-          const uint32_t koff = k * WK * 2;                          // bytes inside the 128 B swizzle row
+          const uint32_t koff = k * WK * 2;                          // bytes inside the 128 B swizzle row (e4m3: k32 steps)
           const uint64_t da_hi = make_smem_desc(sa_hi + koff), db_hi = make_smem_desc(sb_hi + koff);
-          wgmma_tile(acc, da_hi, db_hi, (kb > 0 || k > 0) ? 1u : 0u, FP16);
+          if (E4M3) wgmma_m64n256k32_ss_e4m3(acc, da_hi, db_hi, (kb > 0 || k > 0) ? 1u : 0u);
+          else wgmma_tile(acc, da_hi, db_hi, (kb > 0 || k > 0) ? 1u : 0u, FP16);
           if (NSPLIT == 3) {
             const uint64_t da_lo = make_smem_desc(sa_lo + koff), db_lo = make_smem_desc(sb_lo + koff);
             wgmma_tile(acc, da_hi, db_lo, 1u, false);
@@ -356,8 +373,8 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
       wgmma_wait<0>();
       fence_regs(acc);
       release(prev);
-      if (!second) epilogue_dispatch(p0.ep, acc, rw, col0, p0.N);
-      else epilogue_dispatch(p1.ep, acc, rw, col0, p1.N);
+      if (!second) epilogue_dispatch<E4M3>(p0.ep, acc, rw, col0, p0.N);
+      else epilogue_dispatch<E4M3>(p1.ep, acc, rw, col0, p1.N);
     }
   }
   // ---- teardown: nobody may exit while a peer can still multicast into its shared memory or arrive on its barriers
@@ -376,12 +393,15 @@ bool g_attr_dev[kMaxDev];
 int g_raster_gm = 4;      // SELFTOK_GEMM_GM (measurement knob)
 int g_gemm_ctas = 2;      // 2: two-CTA clusters sharing the W tile (default); 1: one CTA per tile (SELFTOK_GEMM_CTAS=1)
 
-int make_map(CUtensorMap* map, const __nv_bfloat16* ptr, int64_t rows, int K, int box_rows, int fp16) {
+// e4m3: a UINT8 map, 128 elements (the same 128 B) per box row
+int make_map(CUtensorMap* map, const __nv_bfloat16* ptr, int64_t rows, int K, int box_rows, int fp16, bool e4m3 = false) {
   cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)K * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)K * (e4m3 ? 1 : 2)};
+  cuuint32_t box[2] = {(cuuint32_t)(e4m3 ? BK8 : BK), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(map, fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(ptr), gdim, gstride, box, estr,
+  const CUtensorMapDataType dt =
+      e4m3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUresult r = g_encode(map, dt, 2, const_cast<__nv_bfloat16*>(ptr), gdim, gstride, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -452,20 +472,30 @@ int gemm_tc_init() {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   STK_CUDA(cudaDeviceGetAttribute(&g_num_sms_dev[dev], cudaDevAttrMultiProcessorCount, dev));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
-  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3, 1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<3, 2, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<3>::SMEM_BYTES));
+  STK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM_BYTES));
   g_attr_dev[dev] = true;
   return 0;
 }
 
 int check_gemm_tc_problem(const TcProblem& q, int nsplit, int fp16) {
   const Epilogue& ep = q.ep;
+  const bool e4m3 = nsplit == NSPLIT_E4M3;
   STK_CHECK(q.A_hi && q.W_hi && q.M > 0 && q.N > 0 && q.K > 0, -1, "gemm_tc: bad arguments");
-  STK_CHECK(nsplit == 1 || (nsplit == 3 && q.A_lo && q.W_lo), -1, "gemm_tc: nsplit must be 1, or 3 with lo planes");
+  STK_CHECK(nsplit == 1 || e4m3 || (nsplit == 3 && q.A_lo && q.W_lo), -1, "gemm_tc: nsplit must be 1, 3 with lo planes, or e4m3");
+  STK_CHECK(!e4m3 || !fp16, -1, "gemm_tc: e4m3 operands are not IEEE half");
+  STK_CHECK(e4m3 == (ep.s_a != nullptr) && e4m3 == (ep.s_w != nullptr), -1,
+            "gemm_tc: e4m3 problems need both row-scale arrays and 16-bit problems take none (one launch, one operand type)");
+  STK_CHECK(!e4m3 || q.conv_C == 0, -1, "gemm_tc: the e4m3 mode has no convolution");
+  STK_CHECK(!e4m3 || q.K % 16 == 0, -2, "gemm_tc: e4m3 K must be a multiple of 16 (16-byte TMA row pitch)");
+  STK_CHECK(reinterpret_cast<uintptr_t>(ep.s_a) % 4 == 0 && reinterpret_cast<uintptr_t>(ep.s_w) % 8 == 0, -1,
+            "gemm_tc: s_a must be 4-byte and s_w 8-byte aligned");
   STK_CHECK(!fp16 || nsplit == 1, -1, "gemm_tc: the fp16 mode is single-pass");
   auto aligned16 = [](const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; };
   STK_CHECK(aligned16(q.A_hi) && aligned16(q.A_lo) && aligned16(q.W_hi) && aligned16(q.W_lo), -1,
@@ -490,6 +520,12 @@ int check_gemm_tc_problem(const TcProblem& q, int nsplit, int fp16) {
 
 static int make_maps(TcMaps* m, const TcProblem& q, int nsplit, int fp16, int b_box) {
   const bool conv = q.conv_C > 0;
+  if (nsplit == NSPLIT_E4M3) {
+    STK_TRY(make_map(&m->a_hi, q.A_hi, q.M, q.K, BM, 0, true));
+    STK_TRY(make_map(&m->b_hi, q.W_hi, q.N, q.K, b_box, 0, true));
+    m->a_lo = m->a_hi; m->b_lo = m->b_hi;
+    return 0;
+  }
   const int64_t imgs = conv ? q.M / ((int64_t)q.conv_H * q.conv_W) * (q.conv_stride == 2 ? 4 : 1) : 0;   // stride 2: 4 phase planes per image
   if (conv) STK_TRY(make_map_nhwc(&m->a_hi, q.A_hi, imgs, q.conv_H, q.conv_W, q.conv_C, fp16));
   else STK_TRY(make_map(&m->a_hi, q.A_hi, q.M, q.K, BM, fp16));
@@ -504,7 +540,7 @@ static int make_maps(TcMaps* m, const TcProblem& q, int nsplit, int fp16, int b_
   return 0;
 }
 
-template <int NSPLIT, int CL, bool FP16>
+template <int NSPLIT, int CL, bool FP16, bool E4M3>
 static int launch_kernel(const TcMaps& m0, const TcMaps& m1, const GemmParams& p0, const GemmParams& p1, int clusters, cudaStream_t s) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(CL * clusters);
@@ -516,7 +552,7 @@ static int launch_kernel(const TcMaps& m0, const TcMaps& m1, const GemmParams& p
   attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  STK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<NSPLIT, CL, FP16>, m0, m1, p0, p1));
+  STK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<NSPLIT, CL, FP16, E4M3>, m0, m1, p0, p1));
   count_launch();
   return 0;
 }
@@ -524,9 +560,10 @@ static int launch_kernel(const TcMaps& m0, const TcMaps& m1, const GemmParams& p
 template <int CL>
 static int launch_cl(const TcMaps& m0, const TcMaps& m1, const GemmParams& p0, const GemmParams& p1, int clusters, int nsplit, int fp16,
                      cudaStream_t s) {
-  if (nsplit == 3) return launch_kernel<3, CL, false>(m0, m1, p0, p1, clusters, s);
-  if (fp16) return launch_kernel<1, CL, true>(m0, m1, p0, p1, clusters, s);
-  return launch_kernel<1, CL, false>(m0, m1, p0, p1, clusters, s);
+  if (nsplit == NSPLIT_E4M3) return launch_kernel<1, CL, false, true>(m0, m1, p0, p1, clusters, s);
+  if (nsplit == 3) return launch_kernel<3, CL, false, false>(m0, m1, p0, p1, clusters, s);
+  if (fp16) return launch_kernel<1, CL, true, false>(m0, m1, p0, p1, clusters, s);
+  return launch_kernel<1, CL, false, false>(m0, m1, p0, p1, clusters, s);
 }
 
 // One launch for up to two independent problems (the context- and the image-stream GEMM of an MMDiT layer): their tiles share

@@ -17,7 +17,17 @@ namespace stk {
 // plan_ctx = 0 (image stream, rpb_in = N): row r -> c_b + r.
 // Per-row indices (packed step calls, NULL otherwise): tab_rows[m] replaces m % period as the gate / addtab row, and row_map[m]
 // replaces the remap above as the output row.
+// e4m3 operands (NSPLIT_E4M3): A and W hold e4m3 codes with one fp32 scale per row (per GEMM row of A, per output channel of W),
+// and y = act(fma(acc, s_a[m] * s_w[n], bias)) -- the product s_a[m] * s_w[n] rounded to fp32 first, then one fma -- before the
+// mode above.  m is the GEMM row before any remap (plan, row_map, rpb_in), so the scale travels with the A row it belongs to.
+//
+// Quantization contract (per row x of K fp32 values; launch_quant_e4m3_rows, the e4m3 mode of launch_ln_mod_pair):
+//   amax   = max |x_i|, NaN when the row holds a NaN (a NaN-propagating max, never fmaxf)
+//   inv    = __fdiv_rn(448, amax), scale = __fdiv_rn(amax, 448); amax == 0: inv = 0, scale = 0 (all codes 0)
+//   code_i = cvt.rn.satfinite.e4m3(__fmul_rn(x_i, inv))
+// A non-finite amax is not sanitised: the row comes out non-finite downstream.
 enum EpiMode { EPI_STORE = 0, EPI_RESID = 1, EPI_SPLIT = 2 };
+constexpr int NSPLIT_E4M3 = 4;           // launch_gemm_tc* nsplit value of the e4m3 single-pass mode
 struct Epilogue {
   int mode = EPI_STORE;
   int act = 0;
@@ -39,6 +49,8 @@ struct Epilogue {
   int plan_ctx = 0;
   const int* tab_rows = nullptr;         // [M] gate (EPI_RESID) / addtab (EPI_STORE) row of GEMM row m
   const int* row_map = nullptr;          // [M] output row of GEMM row m
+  const float* s_a = nullptr;            // e4m3 only: [M] row scales of A
+  const float* s_w = nullptr;            // e4m3 only: [N] row scales of W (per output channel)
 };
 // slot row of stream row r of an image with plan pair (a, c); n_img = image rows per slot
 __host__ __device__ __forceinline__ int plan_slot_row(int r, int a, int c, int n_img, bool ctx) {
@@ -71,6 +83,8 @@ struct LnProblem {
   __nv_bfloat16* out_lo = nullptr;
   int64_t M = 0;
   const int* rows = nullptr;         // [M] table row of every row (packed step calls; then for every problem of the launch)
+  float* out_scale = nullptr;        // e4m3 output: out_hi holds [M, D] e4m3 codes (D bytes per row) and this [M] fp32 row
+                                     // scales (quantization contract above); then for every problem of the launch
   int imgs = 0;                      // filled by the launcher
 };
 int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStream_t s, int fp16);
@@ -136,6 +150,8 @@ int launch_expand_packed(const int* blk, int B, int K, int N, int S, int* ctx_to
                          int* x_step, cudaStream_t s);
 // zero the rows [c_b + n_img, S) of slot b up to its next 64-row boundary (pair = [B][2] (off_b, c_b)) in a [B*S] x row_bytes buffer
 int launch_zero_slot_tails(const int* pair, int B, int S, int n_img, void* buf, int64_t row_bytes, cudaStream_t s);
+// e4m3 codes [M, K] (K bytes per row) + fp32 scales [M] of fp32 rows x [M, K] under the quantization contract above
+int launch_quant_e4m3_rows(const float* x, int64_t M, int K, uint8_t* codes, float* scales, cudaStream_t s);
 int launch_transpose(const float* in, float* out, int rows, int cols, cudaStream_t s);
 int launch_split_bf16(const float* in, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, cudaStream_t s, int fp16 = 0);
 // out[b, r, :] = src[r, :] for b in 0..B-1 (broadcast rows), optionally + add[r,:]
@@ -147,6 +163,9 @@ int launch_copy_rows(const float* src, int64_t src_bs, float* dst, int64_t dst_b
 // ---- wgmma GEMM (gemm_tc.cu) ----------------------------------------------------------------------------------
 // A planes [M,K] bf16 row-major (lo NULL iff nsplit == 1), W planes [N,K] bf16 row-major.
 // fp16 != 0: operands are IEEE half planes (nsplit must be 1).
+// nsplit == NSPLIT_E4M3: A_hi / W_hi hold e4m3 codes (K bytes per row, K % 16 == 0), lo planes unused, and every problem's
+// epilogue carries both row-scale arrays s_a / s_w (no other mode may carry them, so one launch never mixes operand types).
+// No convolution in this mode.
 int launch_gemm_tc(const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, const __nv_bfloat16* W_hi,
                    const __nv_bfloat16* W_lo, int64_t M, int N, int K, int nsplit, const Epilogue& ep,
                    cudaStream_t s, int fp16 = 0);

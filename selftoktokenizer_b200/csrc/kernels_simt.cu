@@ -329,7 +329,9 @@ struct LnPairParams {
 // the CTA launch itself -- is ~370 of the ~590 instructions a warp spends on its first row.
 // GATHER: every row reads its own table row rows[m] from global memory (packed step calls: rows of one CTA sit at different
 // schedule rows or positions); the arithmetic is the same.
-template <int MAXV, bool FP16, bool LO, bool FULL, int ROWS, bool GATHER>
+// E4M3: out_hi receives e4m3 codes (D bytes per row) and out_scale one fp32 scale per row (the quantization contract of
+// kernels.h): the warp owns the whole row, so the row's amax is one more warp reduction over the modulated values.
+template <int MAXV, bool FP16, bool LO, bool FULL, int ROWS, bool GATHER, bool E4M3>
 __global__ void __launch_bounds__(256) ln_mod_pair_kernel(const LnPairParams p) {
   __shared__ __align__(16) float4 tab[2 * MAXV * 32];
   const bool second = (int)blockIdx.x >= p.nblk0;
@@ -395,6 +397,37 @@ __global__ void __launch_bounds__(256) ln_mod_pair_kernel(const LnPairParams p) 
       __syncthreads();
     }
     if (!active) continue;
+    if (E4M3) {
+      const float4* gsh = GATHER ? reinterpret_cast<const float4*>(q.shift + (int64_t)q.rows[m] * q.ld_mod) : nullptr;
+      const float4* gsc = GATHER ? reinterpret_cast<const float4*>(q.scale + (int64_t)q.rows[m] * q.ld_mod) : nullptr;
+      float amax = 0.f;
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + i * 32;
+        if (FULL || idx < nv) {
+          const float4 h4 = GATHER ? gsh[idx] : tab[idx], s4 = GATHER ? gsc[idx] : tab[MAXV * 32 + idx];
+          float4 y, g;
+          ffma2(v[i].x, v[i].y, rstd, rstd, nmr, nmr, y.x, y.y);
+          ffma2(v[i].z, v[i].w, rstd, rstd, nmr, nmr, y.z, y.w);
+          fadd2(s4.x, s4.y, 1.f, 1.f, g.x, g.y);
+          fadd2(s4.z, s4.w, 1.f, 1.f, g.z, g.w);
+          ffma2(y.x, y.y, g.x, g.y, h4.x, h4.y, y.x, y.y);
+          ffma2(y.z, y.w, g.z, g.w, h4.z, h4.w, y.z, y.w);
+          v[i] = y;                                                    // the modulated row, kept for the second pass
+          amax = fmax_nan(fmax_nan(amax, fabsf(y.x)), fmax_nan(fabsf(y.y), fmax_nan(fabsf(y.z), fabsf(y.w))));
+        }
+      }
+      float inv, scale;
+      e4m3_row_scale(warp_max_nan(amax), inv, scale);
+      uint32_t* oc = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(q.out_hi) + m * (int64_t)p.D);
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + i * 32;
+        if (FULL || idx < nv) oc[idx] = pack4_e4m3(v[i].x, v[i].y, v[i].z, v[i].w, inv);
+      }
+      if (lane == 0) q.out_scale[m] = scale;
+      continue;
+    }
     uint2* oh = reinterpret_cast<uint2*>(q.out_hi + m * (int64_t)p.D);
     uint2* ol = LO ? reinterpret_cast<uint2*>(q.out_lo + m * (int64_t)p.D) : nullptr;
     const float4* gsh = GATHER ? reinterpret_cast<const float4*>(q.shift + (int64_t)q.rows[m] * q.ld_mod) : nullptr;
@@ -439,6 +472,7 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
     return c;
   };
   const bool gather = probs[0].rows != nullptr;
+  const bool e4m3 = probs[0].out_scale != nullptr;
   const int rows = !gather && ctas_for(2) >= 4 * sms ? 2 : 1;
   for (int i = 0; i < 2; ++i) {
     if (i >= n) { p.pr[i] = probs[0]; p.pr[i].M = 0; continue; }
@@ -447,6 +481,9 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
     STK_CHECK(i == 0 || (q.out_lo != nullptr) == lo, -1, "ln_mod_pair: both problems must use the same plane set");
     lo = q.out_lo != nullptr;
     STK_CHECK((q.rows != nullptr) == gather, -1, "ln_mod_pair: per-row table indices must be given for both problems or neither");
+    STK_CHECK((q.out_scale != nullptr) == e4m3, -1, "ln_mod_pair: e4m3 output must be asked for both problems or neither");
+    STK_CHECK(!e4m3 || (!q.out_lo && !fp16 && D % 16 == 0 && reinterpret_cast<uintptr_t>(q.out_hi) % 16 == 0), -1,
+              "ln_mod_pair: e4m3 output has one code plane, D % 16 == 0 and a 16-byte aligned base");
     if (q.period > 1 && !gather) {                                // per-position table: position-major, needs whole images
       STK_CHECK(q.M % q.period == 0, -1, "ln_mod_pair: rows must be whole images of `period` positions");
       q.imgs = (int)(q.M / q.period);
@@ -462,9 +499,10 @@ int launch_ln_mod_pair(const LnProblem* probs, int n, int D, float eps, cudaStre
   const unsigned grid = (unsigned)(nblk[0] + nblk[1]);
 #define STK_LNP3(MAXV, FULL, ROWS, G)                                                          \
   do {                                                                                         \
-    if (fp16) ln_mod_pair_kernel<MAXV, true, false, FULL, ROWS, G><<<grid, 256, 0, s>>>(p);    \
-    else if (lo) ln_mod_pair_kernel<MAXV, false, true, FULL, ROWS, G><<<grid, 256, 0, s>>>(p); \
-    else ln_mod_pair_kernel<MAXV, false, false, FULL, ROWS, G><<<grid, 256, 0, s>>>(p);        \
+    if (e4m3) ln_mod_pair_kernel<MAXV, false, false, FULL, ROWS, G, true><<<grid, 256, 0, s>>>(p);   \
+    else if (fp16) ln_mod_pair_kernel<MAXV, true, false, FULL, ROWS, G, false><<<grid, 256, 0, s>>>(p);    \
+    else if (lo) ln_mod_pair_kernel<MAXV, false, true, FULL, ROWS, G, false><<<grid, 256, 0, s>>>(p); \
+    else ln_mod_pair_kernel<MAXV, false, false, FULL, ROWS, G, false><<<grid, 256, 0, s>>>(p);        \
   } while (0)
 #define STK_LNP(MAXV)                                                                                                      \
   do {                                                                                                                     \
@@ -1092,6 +1130,40 @@ int launch_split_bf16(const float* in, __nv_bfloat16* hi, __nv_bfloat16* lo, int
   STK_CHECK(in && hi && n > 0, -1, "split_bf16: bad arguments");
   int64_t blocks = (n + 255) / 256;
   split_bf16_kernel<<<(unsigned)(blocks > 16384 ? 16384 : blocks), 256, 0, s>>>(in, hi, lo, n, fp16);
+  count_launch();
+  STK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// One warp per row: amax over the row, then the codes (quantization contract of kernels.h).  Weights at finalize and the
+// kernel-level GEMM entry; the decoder's activations are quantized inside ln_mod_pair_kernel.
+__global__ void __launch_bounds__(256) quant_e4m3_rows_kernel(const float* __restrict__ x, int64_t M, int K, uint8_t* __restrict__ codes,
+                                                              float* __restrict__ scales) {
+  const int64_t m = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (m >= M) return;
+  const float4* xr = reinterpret_cast<const float4*>(x + m * K);
+  const int nv = K >> 2;
+  float amax = 0.f;
+  for (int i = lane; i < nv; i += 32) {
+    const float4 v = xr[i];
+    amax = fmax_nan(fmax_nan(amax, fabsf(v.x)), fmax_nan(fabsf(v.y), fmax_nan(fabsf(v.z), fabsf(v.w))));
+  }
+  float inv, scale;
+  e4m3_row_scale(warp_max_nan(amax), inv, scale);
+  uint32_t* cr = reinterpret_cast<uint32_t*>(codes + m * K);
+  for (int i = lane; i < nv; i += 32) {
+    const float4 v = xr[i];
+    cr[i] = pack4_e4m3(v.x, v.y, v.z, v.w, inv);
+  }
+  if (lane == 0) scales[m] = scale;
+}
+
+int launch_quant_e4m3_rows(const float* x, int64_t M, int K, uint8_t* codes, float* scales, cudaStream_t s) {
+  STK_CHECK(x && codes && scales && M > 0 && K > 0 && K % 4 == 0, -1, "quant_e4m3_rows: bad arguments (K % 4 == 0)");
+  STK_CHECK(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(codes) % 4 == 0 && reinterpret_cast<uintptr_t>(scales) % 4 == 0,
+            -1, "quant_e4m3_rows: x must be 16-byte, codes and scales 4-byte aligned");
+  quant_e4m3_rows_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(x, M, K, codes, scales);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;
