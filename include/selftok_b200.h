@@ -208,16 +208,18 @@ int64_t selftok_id_errors(selftok_handle_t h, void* stream);
  * architecture: sd3/sd3_impls.py:314-444.  Weights are loaded under the in-tree SDVAE key names ("decoder.conv_in.weight",
  * "decoder.up.3.block.0.norm1.bias", "encoder.down.0.downsample.conv.weight", ...), fp32, one call per tensor; either half may
  * be omitted (the matching entry point then returns SELFTOK_ERR_MISSING_TENSOR).
- * selftok_vae_decode: z_dev [B,16,h,w] fp32 in VAE latent space (after SD3LatentFormat.process_out), h = w in {8,16,32,64}
- * -> out_dev [B,3,8h,8w] fp32; norm_ip != 0 applies the pipeline's clamp to [-1,1] + rescale to [0,1]. */
+ * selftok_vae_decode: z_dev [B,16,h,w] fp32 in VAE latent space (after SD3LatentFormat.process_out), any 1 <= h, w <= 128
+ * -> out_dev [B,3,8h,8w] fp32; norm_ip != 0 applies the pipeline's clamp to [-1,1] + rescale to [0,1].  Other sizes return
+ * SELFTOK_ERR_UNSUPPORTED before any launch.  Each image's result is independent of the batch it is decoded in. */
 typedef struct selftok_vae* selftok_vae_t;
 int selftok_vae_create(int ch /* 128 */, int device, selftok_vae_t* out);
 int selftok_vae_destroy(selftok_vae_t v);
 int selftok_vae_load_tensor(selftok_vae_t v, const char* name, const void* data, int ndim, const int64_t* shape, int is_device);
 int selftok_vae_finalize(selftok_vae_t v, void* stream);
 int selftok_vae_decode(selftok_vae_t v, const float* z_dev, int B, int h, int w, float* out_dev, int norm_ip, void* stream);
-/* images_dev [B,3,H,W] fp32 in [-1,1], H = W in {128,256,512} -> mean_out_dev [B,16,H/8,W/8] fp32 (the distribution's mode, VAE
- * latent space: apply SD3LatentFormat.process_in afterwards); logvar_out_dev (same shape) may be NULL. */
+/* images_dev [B,3,H,W] fp32 in [-1,1], H and W any multiples of 8 in [8,1024] -> mean_out_dev [B,16,H/8,W/8] fp32 (the
+ * distribution's mode, VAE latent space: apply SD3LatentFormat.process_in afterwards); logvar_out_dev (same shape) may be NULL.
+ * Other sizes return SELFTOK_ERR_UNSUPPORTED before any launch. */
 int selftok_vae_encode(selftok_vae_t v, const float* images_dev, int B, int H, int W, float* mean_out_dev, float* logvar_out_dev,
                        void* stream);
 int64_t selftok_vae_device_bytes(selftok_vae_t v);
@@ -286,6 +288,9 @@ typedef struct selftok_k_gemm_problem {
   int32_t N, K;
   int32_t conv_C, conv_H, conv_W, conv_stride;
   selftok_k_epilogue_t ep;
+  int32_t conv_edge;   /* 0: conv_H / conv_W must be tiled exactly by 128-pixel boxes (part of a row, whole rows of one image, or,
+                        * stride 1 only, whole images), else SELFTOK_ERR_UNSUPPORTED; 1: any geometry -- boxes overhang the right /
+                        * bottom edge and their pixels outside the image are neither stored nor loaded */
 } selftok_k_gemm_problem_t;
 /* path 0: fp32 FFMA kernel, one problem, no convolution (nsplit ignored).  path 1: wgmma kernel, one or two problems in one
  * launch; A / W are converted to 16-bit planes first (nsplit 3: bf16 hi+lo split, 1: bf16, 0: IEEE half single pass), or, with

@@ -58,7 +58,7 @@ class KGemmProblem(C.Structure):
     """selftok_k_gemm_problem_t."""
     _fields_ = [("A", C.c_void_p), ("W", C.c_void_p), ("M", C.c_int64), ("N", C.c_int32), ("K", C.c_int32),
                 ("conv_C", C.c_int32), ("conv_H", C.c_int32), ("conv_W", C.c_int32), ("conv_stride", C.c_int32),
-                ("ep", KEpilogue)]
+                ("ep", KEpilogue), ("conv_edge", C.c_int32)]
 
 
 _lib = None
@@ -581,9 +581,9 @@ class VaeDecoder:
             raise
 
     def decode(self, z: torch.Tensor, norm_ip: bool = False) -> torch.Tensor:
-        """z [B,16,h,w] (VAE latent space) -> [B,3,8h,8w] fp32 on the device."""
-        if z.dim() != 4 or z.shape[1] != 16 or z.shape[2] != z.shape[3]:
-            raise SelftokError(f"VaeDecoder.decode: expected [B,16,h,h] latents, got {tuple(z.shape)}")
+        """z [B,16,h,w] (VAE latent space), 1 <= h, w <= 128 -> [B,3,8h,8w] fp32 on the device."""
+        if z.dim() != 4 or z.shape[1] != 16:
+            raise SelftokError(f"VaeDecoder.decode: expected [B,16,h,w] latents, got {tuple(z.shape)}")
         z = z.to(device=self.device, dtype=torch.float32).contiguous()
         B, _, h, w = z.shape
         out = torch.empty(B, 3, 8 * h, 8 * w, dtype=torch.float32, device=self.device)
@@ -592,10 +592,10 @@ class VaeDecoder:
         return out
 
     def encode(self, images: torch.Tensor, return_logvar: bool = False):
-        """images [B,3,H,H] in [-1,1] -> the latent distribution's mode [B,16,H/8,H/8] fp32 (VAE latent space, before
-        SD3LatentFormat.process_in); with return_logvar also the log-variance."""
-        if images.dim() != 4 or images.shape[1] != 3 or images.shape[2] != images.shape[3]:
-            raise SelftokError(f"VaeDecoder.encode: expected [B,3,H,H] images, got {tuple(images.shape)}")
+        """images [B,3,H,W] in [-1,1], H and W multiples of 8 in [8, 1024] -> the latent distribution's mode [B,16,H/8,W/8] fp32
+        (VAE latent space, before SD3LatentFormat.process_in); with return_logvar also the log-variance."""
+        if images.dim() != 4 or images.shape[1] != 3:
+            raise SelftokError(f"VaeDecoder.encode: expected [B,3,H,W] images, got {tuple(images.shape)}")
         x = images.to(device=self.device, dtype=torch.float32).contiguous()
         B, _, H, W = x.shape
         mean = torch.empty(B, 16, H // 8, W // 8, dtype=torch.float32, device=self.device)
@@ -665,17 +665,18 @@ def _addr(v) -> int:
     return v.data_ptr() if isinstance(v, torch.Tensor) else int(v)
 
 
-def k_gemm_problem(A, W, M, N, K, *, conv=None, mode="store", act="none", **ep) -> KGemmProblem:
+def k_gemm_problem(A, W, M, N, K, *, conv=None, conv_edge=False, mode="store", act="none", **ep) -> KGemmProblem:
     """One selftok_k_gemm_problem_t.  A, W and every pointer field of `ep` (bias, out, resid, gate, addtab, out_hi, out_lo,
     plan, tab_rows, row_map) take a tensor or a raw address; the integer fields (ldo, gate_ld, gate_period, add_ld, add_period,
-    rpb_in, rpb_out, row_off, fp16, plan_ctx) take ints.  conv = (C, H, W, stride) selects the implicit 3x3 convolution."""
+    rpb_in, rpb_out, row_off, fp16, plan_ctx) take ints.  conv = (C, H, W, stride) selects the implicit 3x3 convolution;
+    conv_edge=True lets its 128-pixel tiles overhang the image edge, so that any H, W is accepted."""
     ptrs = ("bias", "out", "resid", "gate", "addtab", "out_hi", "out_lo", "plan", "tab_rows", "row_map")
     e = KEpilogue(mode=_EPI_MODES.get(mode, mode), act=_EPI_ACTS.get(act, act), gate_period=1, add_period=1)
     for k, v in ep.items():
         if k not in dict(KEpilogue._fields_):
             raise TypeError(f"unknown epilogue field {k!r}")
         setattr(e, k, _addr(v) if k in ptrs else int(v))
-    q = KGemmProblem(A=_addr(A), W=_addr(W), M=M, N=N, K=K, ep=e)
+    q = KGemmProblem(A=_addr(A), W=_addr(W), M=M, N=N, K=K, ep=e, conv_edge=int(bool(conv_edge)))
     if conv is not None:
         q.conv_C, q.conv_H, q.conv_W, q.conv_stride = conv
     return q

@@ -1777,6 +1777,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_k_gemm(int path, i
       tp[i] = TcProblem{planes[i][0], planes[i][1], planes[i][2], planes[i][3], q.M, q.N, q.K, eps[i]};
     }
     tp[i].conv_C = q.conv_C; tp[i].conv_H = q.conv_H; tp[i].conv_W = q.conv_W; tp[i].conv_stride = q.conv_stride;
+    tp[i].conv_edge = q.conv_edge;
     st = check_gemm_tc_problem(tp[i], nsplit, fp16);      // shape / geometry errors before any launch
   }
   for (int i = 0; i < n && !st; ++i) {

@@ -60,16 +60,16 @@ struct EpiRows {
   float sa[2];                                         // e4m3: A row scales (GEMM rows, before any remap)
 };
 
+// m[r]: GEMM row of accumulator row r (a convolution's output pixel), valid[r]: m[r] < M and, for a convolution, inside the image
 template <bool E4M3>
-__device__ __forceinline__ EpiRows epilogue_rows(const Epilogue& e, int64_t row0, int64_t M) {
+__device__ __forceinline__ EpiRows epilogue_rows(const Epilogue& e, const int64_t (&m)[2], const bool (&valid)[2]) {
   const bool per_row_gate = e.mode == EPI_RESID && e.gate && (e.gate_period > 1 || e.tab_rows);
   const bool per_row_add = e.mode == EPI_STORE && e.addtab;
   EpiRows rw;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    const int64_t m = row0 + 8 * r;
-    rw.valid[r] = m < M;
-    const int mi = (int)m;
+    rw.valid[r] = valid[r];
+    const int mi = (int)m[r];
     rw.orow[r] = 0;
     if (e.row_map && rw.valid[r]) {
       rw.orow[r] = e.row_map[mi];
@@ -196,14 +196,68 @@ struct GemmParams {
   // implicit-GEMM 3x3 convolution (stride 1, zero padding 1) over NHWC activations: A row m = output pixel (b, y, x), K index =
   // tap * C + c.  conv_C == 0: plain GEMM.  The A tile of k-block kb (tap = kb / (C / 64), channels chunk = kb % (C / 64)) is the
   // 4-D TMA box {64 channels, bw pixels, bh rows, bn images} (bw bh bn = 128) shifted by the tap offset; out-of-image elements
-  // are zero-filled by the TMA unit -- exactly the padding.
+  // are zero-filled by the TMA unit -- exactly the padding.  The 128-row blocks tile each group of bn images as conv_ty x conv_tx
+  // boxes (conv_origin); a box may overhang the right / bottom edge (conv_box), and its rows outside the image are dropped by the
+  // epilogue: no store and no load of resid / gate / addtab.
   // conv_stride == 2 (Downsample, sd3_impls.py:287-298: zero pad right / bottom, 3x3 stride 2): the planes hold the four
   // polyphase components of the input, [image * 4 + (py * 2 + px)][H_out][W_out][C] with phase(py, px)[y][x] = in[2y + py][2x + px];
   // tap (dy, dx) reads phase (dy & 1, dx & 1) shifted by (dy >> 1, dx >> 1) -- unit-stride boxes again, the zero fill past the last
   // row / column is the one-sided padding.  conv_H / conv_W are the OUTPUT dims.
   int conv_C = 0, conv_H = 0, conv_W = 0, conv_stride = 1;
+  int conv_bw = 0, conv_bh = 0, conv_bn = 1, conv_tx = 1, conv_ty = 1;
+  int blocks = 0;        // 128-row A blocks: ceil(M / 128), or images / bn x conv_ty x conv_tx for a convolution
   int raster_gm = 4;     // cluster-rows per raster group (tile_coords)
 };
+
+// first output pixel (b, y, x) of 128-row block `blk` of a convolution
+__device__ __forceinline__ void conv_origin(const GemmParams& p, int blk, int& b, int& y, int& x) {
+  b = blk / (p.conv_tx * p.conv_ty) * p.conv_bn;
+  y = blk / p.conv_tx % p.conv_ty * p.conv_bh;
+  x = blk % p.conv_tx * p.conv_bw;
+}
+
+// Rows lrow and lrow + 8 of 128-row block blk, for one consumer thread's epilogue.  A convolution's row is the output pixel
+// its box element lands on (the box is row-major: x fastest, then y, then image); pixels of an overhanging box that fall
+// outside the image are invalid.  For the boxes that tile images exactly, m = 128 blk + row as in a plain GEMM.
+template <bool E4M3>
+__device__ __forceinline__ EpiRows tile_rows(const GemmParams& p, int blk, int lrow) {
+  int64_t m[2];
+  bool valid[2];
+  if (!E4M3 && p.conv_C > 0) {
+    int b, y, x;
+    conv_origin(p, blk, b, y, x);
+    const int per = p.conv_bw * p.conv_bh;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int l = lrow + 8 * r;
+      const int yy = y + l % per / p.conv_bw, xx = x + l % p.conv_bw;
+      m[r] = ((int64_t)(b + l / per) * p.conv_H + yy) * p.conv_W + xx;
+      valid[r] = yy < p.conv_H && xx < p.conv_W && m[r] < p.M;
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      m[r] = (int64_t)blk * BM + lrow + 8 * r;
+      valid[r] = m[r] < p.M;
+    }
+  }
+  return epilogue_rows<E4M3>(p.ep, m, valid);
+}
+
+// Cluster-row and column tile counts of both problems, problem 0's tile count and the total.  Each role derives them after its
+// setmaxnreg: kept live across it, ptxas spills them.
+struct TileCounts {
+  int pm0, n0, pm1, n1, tiles0, total;
+};
+template <int CL>
+__device__ __forceinline__ TileCounts tile_counts(const GemmParams& p0, const GemmParams& p1) {
+  TileCounts c;
+  c.pm0 = (p0.blocks + CL - 1) / CL; c.n0 = (p0.N + BN - 1) / BN;
+  c.pm1 = (p1.blocks + CL - 1) / CL; c.n1 = (p1.N + BN - 1) / BN;
+  c.tiles0 = c.pm0 * c.n0;
+  c.total = c.tiles0 + c.pm1 * c.n1;
+  return c;
+}
 
 __device__ __forceinline__ void tile_coords(int t, int pm_tiles, int n_tiles, int GM, int& pm, int& n_blk) {
   // GM cluster-rows share each W tile in L2; SELFTOK_GEMM_GM is a measurement knob (any value is a bijection of the tile
@@ -239,10 +293,6 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = CL > 1 ? cluster_ctarank() : 0;
-  const int pm_tiles0 = (int)((p0.M + CL * BM - 1) / (CL * BM)), n_tiles0 = (p0.N + BN - 1) / BN;
-  const int pm_tiles1 = (int)((p1.M + CL * BM - 1) / (CL * BM)), n_tiles1 = (p1.N + BN - 1) / BN;
-  const int tiles0 = pm_tiles0 * n_tiles0;
-  const int num_tiles = tiles0 + pm_tiles1 * n_tiles1;
   const int cluster_id = blockIdx.x / CL, num_clusters = gridDim.x / CL;
 
   if (warp == CONSUMERS * 4 && lane == 0) {
@@ -263,6 +313,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
   if (warp >= CONSUMERS * 4) {
     // =========================================================== TMA producer
     setmaxnreg_dec<PRODUCER_REGS>();
+    const auto [pm_tiles0, n_tiles0, pm_tiles1, n_tiles1, tiles0, num_tiles] = tile_counts<CL>(p0, p1);
     if (warp == CONSUMERS * 4 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       // The weight tile is re-read by every group of M tiles; without a hint the activation / residual / output streams of the
@@ -276,23 +327,22 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
         if (second) tile_coords(t - tiles0, pm_tiles1, n_tiles1, p1.raster_gm, pm, n_blk);
         else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
         const int nk = (pp.K + KB - 1) / KB;
-        const int m_row = (pm * CL + (int)rank) * BM;               // this CTA's 128 A rows
+        const int blk = pm * CL + (int)rank;                        // this CTA's 128 A rows
+        const int m_row = blk * BM;
         const int n_row = n_blk * BN + (int)rank * (BN / CL);       // this CTA's share of the W tile
-        // convolution: the 128 rows are 128 / bw image rows of bw pixels starting at (cb, cy, cx)
-        const int chunks = pp.conv_C > 0 ? pp.conv_C / BK : 1;
+        // convolution: the 128 rows are the box of bh image rows of bw pixels (of bn images) starting at (cb, cy, cx)
+        // (the e4m3 mode has no convolution: the host refuses it, and its instantiations carry no convolution code)
+        const bool conv = !E4M3 && pp.conv_C > 0;
+        const int chunks = conv ? pp.conv_C / BK : 1;
         int cx = 0, cy = 0, cb = 0;
-        if (pp.conv_C > 0) {
-          cx = m_row % pp.conv_W;
-          cy = (m_row / pp.conv_W) % pp.conv_H;
-          cb = m_row / (pp.conv_W * pp.conv_H);
-        }
+        if (conv) conv_origin(pp, blk, cb, cy, cx);
         for (int kb = 0; kb < nk; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1);
           const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
           const uint32_t sb = sa + C::PLANES * A_TILE_BYTES + (uint32_t)rank * (B_TILE_BYTES / CL);
           const uint32_t fb = full_bar(stage);
           mbar_expect_tx(fb, C::STAGE_BYTES);
-          if (pp.conv_C > 0) {
+          if (conv) {
             const int tap = kb / chunks, c0 = (kb - tap * chunks) * BK;
             const int dy = tap / 3, dx = tap - dy * 3;
             int x0 = cx + dx - 1, y0 = cy + dy - 1, n0 = cb;
@@ -317,6 +367,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
   } else {
     // =========================================================== consumer warpgroups: wgmma + epilogue
     setmaxnreg_inc<CONSUMER_REGS>();
+    const auto [pm_tiles0, n_tiles0, pm_tiles1, n_tiles1, tiles0, num_tiles] = tile_counts<CL>(p0, p1);
     const int wg = warp >> 2;                                        // rows [64 wg, 64 wg + 64) of the CTA's 128
     const bool signaller = (threadIdx.x & 127) == 0;
     auto release = [&](int s) {                                      // the stage's wgmma reads have completed
@@ -332,10 +383,10 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps0, const __grid_constant__ TcM
       else tile_coords(t, pm_tiles0, n_tiles0, p0.raster_gm, pm, n_blk);
       const int nk = ((second ? p1.K : p0.K) + KB - 1) / KB;
       const int wl = threadIdx.x & 127;
-      const int64_t row0 = (int64_t)(pm * CL + (int)rank) * BM + wg * 64 + (wl >> 5) * 16 + ((wl & 31) >> 2);
+      const int blk = pm * CL + (int)rank, lrow = wg * 64 + (wl >> 5) * 16 + ((wl & 31) >> 2);
       const int col0 = n_blk * BN + 2 * (wl & 3);
       // the two problems are handled by separate (statically addressed) copies of the epilogue
-      const EpiRows rw = second ? epilogue_rows<E4M3>(p1.ep, row0, p1.M) : epilogue_rows<E4M3>(p0.ep, row0, p0.M);
+      const EpiRows rw = second ? tile_rows<E4M3>(p1, blk, lrow) : tile_rows<E4M3>(p0, blk, lrow);
       const int pf_kb = nk > kPrefetchKBlocks ? nk - kPrefetchKBlocks : 0;
       float acc[ACC];
 #pragma unroll
@@ -411,12 +462,41 @@ int make_map(CUtensorMap* map, const __nv_bfloat16* ptr, int64_t rows, int K, in
   return 0;
 }
 
-// 4-D map over NHWC 16-bit activations [B][H][W][C] with box {64 channels, bw pixels, bh rows, 128 / (bw bh) images}: 128 output
-// pixels per CTA = part of an image row (W >= 128), whole rows of one image, or -- for images smaller than 128 pixels -- whole images
-int make_map_nhwc(CUtensorMap* map, const __nv_bfloat16* ptr, int64_t B, int H, int W, int Cc, int fp16) {
-  const int bw = W < BM ? W : BM;
-  const int bh = (BM / bw) < H ? (BM / bw) : H;
-  const int bn = BM / (bw * bh);
+// The A box {64 channels, bw pixels, bh rows, bn images} (bw bh bn = 128) of a convolution with output dims H x W, and the
+// ty x tx boxes that cover one group of bn images.  It depends on the geometry alone, never on the batch, so an image's result
+// does not depend on the images launched with it.  An exact box is part of an image row (W a multiple of 128), whole rows of one
+// image, or whole images; stride 2 needs bn = 1, because consecutive planes are the phases of one image.  Without one, `edge`
+// allows bn = 1 and the power-of-two bw x bh with the fewest boxes per image (the wider on a tie), overhanging the right and
+// bottom edges; the TMA zero fill supplies the padding and the overhang alike.  Returns false when no box is allowed.
+struct ConvBox {
+  int bw, bh, bn, tx, ty;
+};
+bool conv_box(int H, int W, int stride, bool edge, ConvBox& bx) {
+  const int64_t hw = (int64_t)H * W;
+  const bool exact = (W % BM == 0 || BM % W == 0) && (hw % BM == 0 || BM % hw == 0) &&
+                     (W >= BM || hw < BM || H % (BM / W) == 0) && (stride == 1 || hw % BM == 0);
+  if (exact) {
+    bx.bw = W < BM ? W : BM;
+    bx.bh = (BM / bx.bw) < H ? (BM / bx.bw) : H;
+    bx.bn = BM / (bx.bw * bx.bh);
+  } else {
+    if (!edge) return false;
+    int64_t best = -1;
+    for (int bw = BM; bw >= 1; bw /= 2) {
+      const int bh = BM / bw;
+      const int64_t n = (int64_t)((W + bw - 1) / bw) * ((H + bh - 1) / bh);
+      if (best < 0 || n < best) { best = n; bx.bw = bw; bx.bh = bh; }
+    }
+    bx.bn = 1;
+  }
+  bx.tx = (W + bx.bw - 1) / bx.bw;
+  bx.ty = (H + bx.bh - 1) / bx.bh;
+  return true;
+}
+
+// 4-D map over NHWC 16-bit activations [B][H][W][C] with the box {64 channels, bw pixels, bh rows, bn images}
+int make_map_nhwc(CUtensorMap* map, const __nv_bfloat16* ptr, int64_t B, int H, int W, int Cc, int fp16, const ConvBox& bx) {
+  const int bw = bx.bw, bh = bx.bh, bn = bx.bn;
   cuuint64_t gdim[4] = {(cuuint64_t)Cc, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   cuuint64_t gstride[3] = {(cuuint64_t)Cc * 2, (cuuint64_t)W * Cc * 2, (cuuint64_t)H * W * Cc * 2};
   cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
@@ -509,11 +589,12 @@ int check_gemm_tc_problem(const TcProblem& q, int nsplit, int fp16) {
   STK_CHECK(ep.mode != EPI_RESID || ep.gate == nullptr || ep.gate_ld % 4 == 0, -2, "gemm_tc: gate pitch must be a multiple of 4");
   if (q.conv_C > 0) {                                      // implicit 3x3 convolution over NHWC planes
     STK_CHECK(q.conv_C % BK == 0 && q.K == 9 * q.conv_C, -2, "gemm_tc conv: channels must be a multiple of 64 and K = 9 C");
-    STK_CHECK(q.conv_W > 0 && q.conv_H > 0 && (q.conv_W % BM == 0 || BM % q.conv_W == 0), -2, "gemm_tc conv: image width must divide or be a multiple of 128");
-    const int64_t hw = (int64_t)q.conv_H * q.conv_W;
-    STK_CHECK(q.M % hw == 0 && (hw % BM == 0 || BM % hw == 0) && (q.conv_W >= BM || hw < BM || q.conv_H % (BM / q.conv_W) == 0), -2,
-              "gemm_tc conv: 128-pixel tiles must be part of a row, whole rows of one image, or whole images");
-    STK_CHECK(q.conv_stride == 1 || (q.conv_stride == 2 && hw % BM == 0), -2, "gemm_tc conv: stride 2 needs >= 128 output pixels per image");
+    STK_CHECK(q.conv_W > 0 && q.conv_H > 0 && (q.conv_stride == 1 || q.conv_stride == 2), -2, "gemm_tc conv: bad geometry or stride");
+    STK_CHECK(q.M % ((int64_t)q.conv_H * q.conv_W) == 0, -2, "gemm_tc conv: M must be a whole number of images");
+    ConvBox bx;
+    STK_CHECK(conv_box(q.conv_H, q.conv_W, q.conv_stride, q.conv_edge != 0, bx), -2,
+              "gemm_tc conv: without conv_edge, 128-pixel tiles must be part of a row, whole rows of one image, or whole images "
+              "(stride 2: no whole images)");
   }
   return 0;
 }
@@ -527,11 +608,13 @@ static int make_maps(TcMaps* m, const TcProblem& q, int nsplit, int fp16, int b_
     return 0;
   }
   const int64_t imgs = conv ? q.M / ((int64_t)q.conv_H * q.conv_W) * (q.conv_stride == 2 ? 4 : 1) : 0;   // stride 2: 4 phase planes per image
-  if (conv) STK_TRY(make_map_nhwc(&m->a_hi, q.A_hi, imgs, q.conv_H, q.conv_W, q.conv_C, fp16));
+  ConvBox bx{};
+  if (conv) conv_box(q.conv_H, q.conv_W, q.conv_stride, q.conv_edge != 0, bx);     // accepted by check_gemm_tc_problem
+  if (conv) STK_TRY(make_map_nhwc(&m->a_hi, q.A_hi, imgs, q.conv_H, q.conv_W, q.conv_C, fp16, bx));
   else STK_TRY(make_map(&m->a_hi, q.A_hi, q.M, q.K, BM, fp16));
   STK_TRY(make_map(&m->b_hi, q.W_hi, q.N, q.K, b_box, fp16));
   if (nsplit == 3) {
-    if (conv) STK_TRY(make_map_nhwc(&m->a_lo, q.A_lo, imgs, q.conv_H, q.conv_W, q.conv_C, fp16));
+    if (conv) STK_TRY(make_map_nhwc(&m->a_lo, q.A_lo, imgs, q.conv_H, q.conv_W, q.conv_C, fp16, bx));
     else STK_TRY(make_map(&m->a_lo, q.A_lo, q.M, q.K, BM, fp16));
     STK_TRY(make_map(&m->b_lo, q.W_lo, q.N, q.K, b_box, fp16));
   } else {
@@ -581,18 +664,27 @@ int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream
   auto mk_params = [&](const TcProblem& q) {
     GemmParams g{q.M, q.N, q.K, fp16, q.ep};
     g.conv_C = q.conv_C; g.conv_H = q.conv_H; g.conv_W = q.conv_W; g.conv_stride = q.conv_stride;
+    g.blocks = (int)((q.M + BM - 1) / BM);
+    ConvBox bx;
+    if (q.conv_C > 0 && conv_box(q.conv_H, q.conv_W, q.conv_stride, q.conv_edge != 0, bx)) {
+      const int64_t imgs = q.M / ((int64_t)q.conv_H * q.conv_W);
+      g.conv_bw = bx.bw; g.conv_bh = bx.bh; g.conv_bn = bx.bn; g.conv_tx = bx.tx; g.conv_ty = bx.ty;
+      g.blocks = (int)((imgs + bx.bn - 1) / bx.bn * bx.ty * bx.tx);
+    }
     g.raster_gm = g_raster_gm;
     return g;
   };
+  auto tiles_of = [&](const GemmParams& g) { return (g.blocks + CL - 1) / CL * ((g.N + BN - 1) / BN); };
   GemmParams p0 = mk_params(probs[0]);
   GemmParams p1 = p0;
   p1.M = 0;
+  p1.blocks = 0;
   m1 = m0;
-  int tiles = (int)((probs[0].M + CL * BM - 1) / (CL * BM)) * ((probs[0].N + BN - 1) / BN);
+  int tiles = tiles_of(p0);
   if (n == 2) {
     STK_TRY(make_maps(&m1, probs[1], nsplit, fp16, BN / CL));
     p1 = mk_params(probs[1]);
-    tiles += (int)((probs[1].M + CL * BM - 1) / (CL * BM)) * ((probs[1].N + BN - 1) / BN);
+    tiles += tiles_of(p1);
   }
   const int clusters = tiles < g_num_sms / CL ? tiles : g_num_sms / CL;
   if (CL == 2) return launch_cl<2>(m0, m1, p0, p1, clusters, nsplit, fp16, s);

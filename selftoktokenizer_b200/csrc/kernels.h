@@ -175,8 +175,10 @@ struct TcProblem {
   Epilogue ep;
   // conv_C > 0: implicit-GEMM 3x3 convolution (stride 1, pad 1): A planes are NHWC activations [M / (H W), H, W, C], W planes
   // [N, 9 C] with K index = (ky * 3 + kx) * C + c, M = output pixels, K = 9 C.  conv_stride == 2: A planes are the four
-  // polyphase components of the input [images * 4, H_out, W_out, C] (pad right / bottom), conv_H / conv_W = output dims
-  int conv_C = 0, conv_H = 0, conv_W = 0, conv_stride = 1;
+  // polyphase components of the input [images * 4, H_out, W_out, C] (pad right / bottom), conv_H / conv_W = output dims.
+  // conv_edge == 0: the 128-pixel A tiles must tile each image exactly (part of a row, whole rows, or whole images; stride 2: not
+  // whole images); != 0: any H, W -- tiles then overhang the right / bottom edge and their outside rows are dropped.
+  int conv_C = 0, conv_H = 0, conv_W = 0, conv_stride = 1, conv_edge = 0;
 };
 // one launch for one or two independent problems of the same operand type
 int launch_gemm_tc_grouped(const TcProblem* probs, int n, int nsplit, cudaStream_t s, int fp16 = 0);

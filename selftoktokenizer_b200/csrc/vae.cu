@@ -12,6 +12,7 @@
 //   3x3 convs     implicit GEMM on the wgmma kernel of gemm_tc.cu: A tile = 4-D TMA box of the NHWC planes shifted by
 //                 the tap offset (the TMA unit's out-of-bounds zero fill IS the padding), K = 9 C, weights repacked to
 //                 [Cout, (ky, kx), Cin]; bias and the residual add (x + h, ResnetBlock.forward :256) in the GEMM epilogue.
+//                 Any image size: where no 128-pixel box tiles the image exactly, the boxes overhang its right / bottom edge.
 //   stride-2 conv the input is written as its four polyphase planes (space_to_depth_planes_kernel); every tap is then a
 //                 unit-stride box of one phase plane, and the zero fill past the last row / column is the one-sided padding.
 //   GroupNorm     32 groups, eps 1e-6, affine; two deterministic passes (per-chunk partial sums in a fixed order, then
@@ -153,13 +154,14 @@ __global__ void __launch_bounds__(256) space_to_depth_planes_kernel(const float*
     reinterpret_cast<uint2*>(lo)[i] = make_uint2(pack2_resid_bf16(v.x, v.y, p0), pack2_resid_bf16(v.z, v.w, p1));
   }
 }
-// row softmax of the attention scores: P = softmax(S * scale) [rows, n] fp32 -> bf16 hi / lo planes; one warp per row
+// row softmax of the attention scores: P = softmax(S * scale) over the n real columns of S [rows, ld] fp32 -> bf16 hi / lo
+// planes [rows, ld] whose columns [n, ld) (the pad to a 16-byte row pitch) are zero; one warp per row
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ s, bf16* __restrict__ hi, bf16* __restrict__ lo, int64_t rows, int n,
-                                                           float scale) {
+                                                           int ld, float scale) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
-  const float* sr = s + row * n;
+  const float* sr = s + row * ld;
   float mx = -INFINITY;
   for (int i = lane; i < n; i += 32) mx = fmaxf(mx, sr[i]);
   mx = warp_max(mx) * scale;
@@ -170,8 +172,12 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
     const float p = expf(sr[i] * scale - mx) * inv;
     uint16_t a, r;
     split16(p, false, a, r);
-    reinterpret_cast<uint16_t*>(hi)[row * n + i] = a;
-    reinterpret_cast<uint16_t*>(lo)[row * n + i] = r;
+    reinterpret_cast<uint16_t*>(hi)[row * ld + i] = a;
+    reinterpret_cast<uint16_t*>(lo)[row * ld + i] = r;
+  }
+  for (int i = n + lane; i < ld; i += 32) {
+    reinterpret_cast<uint16_t*>(hi)[row * ld + i] = 0;
+    reinterpret_cast<uint16_t*>(lo)[row * ld + i] = 0;
   }
 }
 // conv_out result [B, H, W, 4] fp32 NHWC (3 real channels) -> [B, 3, H, W] NCHW, optionally norm_ip(., -1, 1) (clamp to [-1, 1],
@@ -223,8 +229,8 @@ struct selftok_vae {
   std::unordered_map<std::string, std::pair<float*, std::vector<int64_t>>> raw;      // loaded fp32 tensors (freed at finalize unless norm / bias)
   std::unordered_map<std::string, VaeW> conv;
   std::vector<void*> allocs;
-  // workspace (sized for the largest batch / latent side seen)
-  int wsB = 0, wsh = 0;
+  // workspace (sized for the last batch / latent size that did not fit the one before)
+  int wsB = 0, wsh = 0, wsw = 0;
   std::vector<void*> ws_allocs;
   float *xa = nullptr, *xb = nullptr, *sc = nullptr, *part = nullptr, *stats = nullptr, *s_attn = nullptr, *out4 = nullptr;
   bf16 *p_hi = nullptr, *p_lo = nullptr, *q_hi = nullptr, *q_lo = nullptr, *k_hi = nullptr, *k_lo = nullptr, *vt_hi = nullptr, *vt_lo = nullptr,
@@ -389,7 +395,9 @@ static const float* vget(selftok_vae* v, const std::string& name) {
   auto it = v->raw.find(name);
   return it == v->raw.end() ? nullptr : it->second.first;
 }
-// y = conv(planes) (+ resid) -> out (fp32 NHWC [M, N]); taps == 9: implicit GEMM over [B, H, W, Cpad] planes
+// y = conv(planes) (+ resid) -> out (fp32 NHWC [M, N]); taps == 9: implicit GEMM over [B, H, W, Cpad] planes, at any H, W (its
+// 128-pixel tiles may overhang the image edge; their outside rows are neither stored nor loaded, so the fp32 stream only ever
+// holds the H W real pixels of each image)
 static int vconv(VaeCtx& c, const std::string& name, const bf16* a_hi, const bf16* a_lo, int H, int W, float* out, const float* resid, int stride = 1) {
   auto it = c.v->conv.find(name);
   STK_CHECK(it != c.v->conv.end(), SELFTOK_ERR_STATE, "VAE conv not packed");
@@ -398,10 +406,12 @@ static int vconv(VaeCtx& c, const std::string& name, const bf16* a_hi, const bf1
   ep.bias = w.bias; ep.out = out; ep.ldo = w.Npad;
   if (resid) { ep.mode = EPI_RESID; ep.resid = resid; }
   TcProblem q{a_hi, a_lo, w.hi, w.lo, (int64_t)c.B * H * W, w.Npad, w.K, ep};
-  if (w.taps == 9) { q.conv_C = w.Cpad; q.conv_H = H; q.conv_W = W; q.conv_stride = stride; }      // stride 2: H, W = output dims
+  if (w.taps == 9) { q.conv_C = w.Cpad; q.conv_H = H; q.conv_W = W; q.conv_stride = stride; q.conv_edge = 1; }   // stride 2: H, W = output dims
   return launch_gemm_tc_grouped(&q, 1, 3, c.s, 0);
 }
-// GroupNorm (+ SiLU) of the fp32 NHWC stream x [B, HW, C] into the operand planes
+// GroupNorm (+ SiLU) of the fp32 NHWC stream x [B, HW, C] into the operand planes.  The statistics cover exactly the H W real
+// pixels of each image: the stream is dense [B, H, W, C], and the rows of a convolution tile that overhang the image edge
+// never reach it (vconv).
 static int vnorm(VaeCtx& c, const std::string& name, const float* x, int64_t HW, int C, bool silu_act) {
   selftok_vae* v = c.v;
   const float *g = vget(v, name + ".weight"), *b = vget(v, name + ".bias");
@@ -447,7 +457,11 @@ static int vmid(VaeCtx& c, const std::string& pre, float*& x, float*& y, int H, 
   STK_TRY(vresnet(c, pre + ".mid.block_1", x, y, H, W, Cm, Cm));
   {
     // AttnBlock (sd3_impls.py:276-287): h = norm(x); q, k, v = 1x1 convs; softmax(q k^T / sqrt(C)) v; x + proj_out(.)
-    const int64_t T = (int64_t)H * W;
+    // The key axis of S, P and V^T is padded to Tp, a multiple of 8 (16-byte rows for TMA and the GEMM pitch checks).  S's pad
+    // columns are products with the rows after image b's keys (the next image's, or the workspace's slack rows) and are never
+    // read; P's pad columns are written as zero by the softmax and V^T's are cleared, so that they add exactly 0 to P V (0 x NaN
+    // would be NaN).
+    const int64_t T = (int64_t)H * W, Tp = (T + 7) / 8 * 8;
     STK_TRY(vnorm(c, pre + ".mid.attn_1.norm", x, T, Cm, false));
     auto lin_planes = [&](const std::string& name, bf16* oh, bf16* ol) -> int {       // [B T, C] planes -> [B T, C] planes (+ bias)
       const VaeW& wq = v->conv[name];
@@ -460,23 +474,27 @@ static int vmid(VaeCtx& c, const std::string& pre, float*& x, float*& y, int H, 
     STK_TRY(lin_planes(pre + ".mid.attn_1.k", v->k_hi, v->k_lo));
     const VaeW& wv = v->conv[pre + ".mid.attn_1.v"];
     for (int b = 0; b < B; ++b) {
-      const int64_t off = (int64_t)b * T * Cm;
-      // V^T [C, T] = W_v [C, C] . h_b^T  (operands swapped; the bias is added after P V: the rows of P sum to one)
+      const int64_t off = (int64_t)b * T * Cm, off_vt = (int64_t)b * Cm * Tp;
+      // V^T [C, Tp] = W_v [C, C] . h_b^T  (operands swapped; the bias is added after P V: the rows of P sum to one)
       Epilogue ev;
-      ev.mode = EPI_SPLIT; ev.out_hi = v->vt_hi + off; ev.out_lo = v->vt_lo + off; ev.ldo = T;
-      TcProblem qv{wv.hi, wv.lo, v->p_hi + off, v->p_lo + off, Cm, (int)T, Cm, ev};
+      ev.mode = EPI_SPLIT; ev.out_hi = v->vt_hi + off_vt; ev.out_lo = v->vt_lo + off_vt; ev.ldo = Tp;
+      TcProblem qv{wv.hi, wv.lo, v->p_hi + off, v->p_lo + off, Cm, (int)Tp, Cm, ev};
       STK_TRY(launch_gemm_tc_grouped(&qv, 1, 3, s, 0));
-      // S = Q_b K_b^T  [T, T] fp32
+      if (Tp > T) {
+        STK_CUDA(cudaMemset2DAsync(v->vt_hi + off_vt + T, Tp * sizeof(bf16), 0, (Tp - T) * sizeof(bf16), Cm, s));
+        STK_CUDA(cudaMemset2DAsync(v->vt_lo + off_vt + T, Tp * sizeof(bf16), 0, (Tp - T) * sizeof(bf16), Cm, s));
+      }
+      // S = Q_b K_b^T  [T, Tp] fp32
       Epilogue es;
-      es.out = v->s_attn; es.ldo = T;
-      TcProblem qs{v->q_hi + off, v->q_lo + off, v->k_hi + off, v->k_lo + off, T, (int)T, Cm, es};
+      es.out = v->s_attn; es.ldo = Tp;
+      TcProblem qs{v->q_hi + off, v->q_lo + off, v->k_hi + off, v->k_lo + off, T, (int)Tp, Cm, es};
       STK_TRY(launch_gemm_tc_grouped(&qs, 1, 3, s, 0));
-      softmax_rows_kernel<<<(unsigned)((T + 7) / 8), 256, 0, s>>>(v->s_attn, v->pr_hi, v->pr_lo, T, (int)T, 1.0f / sqrtf((float)Cm));
+      softmax_rows_kernel<<<(unsigned)((T + 7) / 8), 256, 0, s>>>(v->s_attn, v->pr_hi, v->pr_lo, T, (int)T, (int)Tp, 1.0f / sqrtf((float)Cm));
       count_launch();
       // O_b = P V + b_v  [T, C] -> planes (A operand of proj_out)
       Epilogue eo;
       eo.mode = EPI_SPLIT; eo.bias = wv.bias; eo.out_hi = v->o_hi + off; eo.out_lo = v->o_lo + off; eo.ldo = Cm;
-      TcProblem qo{v->pr_hi, v->pr_lo, v->vt_hi + off, v->vt_lo + off, T, Cm, (int)T, eo};
+      TcProblem qo{v->pr_hi, v->pr_lo, v->vt_hi + off_vt, v->vt_lo + off_vt, T, Cm, (int)Tp, eo};
       STK_TRY(launch_gemm_tc_grouped(&qo, 1, 3, s, 0));
     }
     STK_TRY(vconv(c, pre + ".mid.attn_1.proj_out", v->o_hi, v->o_lo, H, W, y, x));     // y = x + proj_out(o)
@@ -486,21 +504,25 @@ static int vmid(VaeCtx& c, const std::string& pre, float*& x, float*& y, int H, 
   return 0;
 }
 
-static int vae_ensure_ws(selftok_vae* v, int B, int h) {
-  if (v->wsB >= B && v->wsh >= h) return 0;
+// workspace for B images of latent size h x w (a decode of [B, 16, h, w], or an encode of [B, 3, 8h, 8w]); kept while a call fits
+static int vae_ensure_ws(selftok_vae* v, int B, int h, int w) {
+  if (v->wsB >= B && v->wsh >= h && v->wsw >= w) return 0;
   for (void* p : v->ws_allocs) cudaFree(p);
   v->ws_allocs.clear();
   auto& P = v->ws_allocs;
   const int ch = v->ch;
-  // the largest fp32 tensor: max over levels of H W C (level l: side h * 2^(3-l), channels ch * mult[l]); and the padded conv_in input
-  int64_t big = (int64_t)h * h * 64;
+  // the largest fp32 tensor: max over levels of H W C (level l: h * 2^(3-l) x w * 2^(3-l), channels ch * mult[l]); and the
+  // padded conv_in input
+  int64_t big = (int64_t)h * w * 64;
   for (int l = 0; l < 4; ++l) {
-    const int64_t side = (int64_t)h << (3 - l);
-    big = std::max(big, side * side * ch * v->mult[l]);
-    if (l > 0) big = std::max(big, (side * 2) * (side * 2) * ch * v->mult[l]);       // upsampled planes keep the level's channels
+    const int64_t hs = (int64_t)h << (3 - l), ws = (int64_t)w << (3 - l);
+    big = std::max(big, hs * ws * ch * v->mult[l]);
+    if (l > 0) big = std::max(big, (hs * 2) * (ws * 2) * ch * v->mult[l]);           // upsampled planes keep the level's channels
   }
   big *= B;
-  const int64_t T = (int64_t)h * h, Cm = (int64_t)ch * v->mult[3];
+  // attention (vmid): key axis padded to Tp; the S and V^T GEMMs read Tp rows of image b's keys / normalised input, so the last
+  // image reads up to 7 rows past B T: k gets 8 slack rows, and the p planes (big >= B 8h 8w 128 = 16 B T Cm) have them already
+  const int64_t T = (int64_t)h * w, Tp = (T + 7) / 8 * 8, Cm = (int64_t)ch * v->mult[3];
   STK_TRY(v_alloc_t(v, P, &v->xa, big));
   STK_TRY(v_alloc_t(v, P, &v->xb, big));
   STK_TRY(v_alloc_t(v, P, &v->sc, big));
@@ -508,34 +530,35 @@ static int vae_ensure_ws(selftok_vae* v, int B, int h) {
   STK_TRY(v_alloc_t(v, P, &v->p_lo, big));
   STK_TRY(v_alloc_t(v, P, &v->q_hi, big));
   STK_TRY(v_alloc_t(v, P, &v->q_lo, big));
-  STK_TRY(v_alloc_t(v, P, &v->k_hi, (int64_t)B * T * Cm));
-  STK_TRY(v_alloc_t(v, P, &v->k_lo, (int64_t)B * T * Cm));
-  STK_TRY(v_alloc_t(v, P, &v->vt_hi, (int64_t)B * T * Cm));
-  STK_TRY(v_alloc_t(v, P, &v->vt_lo, (int64_t)B * T * Cm));
-  STK_TRY(v_alloc_t(v, P, &v->pr_hi, T * T));
-  STK_TRY(v_alloc_t(v, P, &v->pr_lo, T * T));
+  STK_TRY(v_alloc_t(v, P, &v->k_hi, ((int64_t)B * T + 8) * Cm));
+  STK_TRY(v_alloc_t(v, P, &v->k_lo, ((int64_t)B * T + 8) * Cm));
+  STK_TRY(v_alloc_t(v, P, &v->vt_hi, (int64_t)B * Cm * Tp));
+  STK_TRY(v_alloc_t(v, P, &v->vt_lo, (int64_t)B * Cm * Tp));
+  STK_TRY(v_alloc_t(v, P, &v->pr_hi, T * Tp));
+  STK_TRY(v_alloc_t(v, P, &v->pr_lo, T * Tp));
   STK_TRY(v_alloc_t(v, P, &v->o_hi, (int64_t)B * T * Cm));
   STK_TRY(v_alloc_t(v, P, &v->o_lo, (int64_t)B * T * Cm));
-  STK_TRY(v_alloc_t(v, P, &v->s_attn, T * T));
-  const int64_t HWmax = ((int64_t)h * 8) * ((int64_t)h * 8);
+  STK_TRY(v_alloc_t(v, P, &v->s_attn, T * Tp));
+  const int64_t HWmax = ((int64_t)h * 8) * ((int64_t)w * 8);
   STK_TRY(v_alloc_t(v, P, &v->part, (int64_t)B * ((HWmax + 1023) / 1024) * 2 * GN_GROUPS));
   STK_TRY(v_alloc_t(v, P, &v->stats, (int64_t)B * GN_GROUPS * 2));
   STK_TRY(v_alloc_t(v, P, &v->out4, (int64_t)B * HWmax * 4));
-  v->wsB = B; v->wsh = h;
+  v->wsB = B; v->wsh = h; v->wsw = w;
   return 0;
 }
 
-// z_dev [B, 16, h, w] fp32 (VAE latent space, i.e. AFTER SD3LatentFormat.process_out) -> out_dev [B, 3, 8h, 8w] fp32;
-// norm_ip != 0: clamp to [-1, 1] and rescale to [0, 1] (SelftokPipeline.py:293).
+// z_dev [B, 16, h, w] fp32 (VAE latent space, i.e. AFTER SD3LatentFormat.process_out), 1 <= h, w <= 128 -> out_dev [B, 3, 8h, 8w]
+// fp32; norm_ip != 0: clamp to [-1, 1] and rescale to [0, 1] (SelftokPipeline.py:293).  Each image's result does not depend on
+// the batch: every kernel works per pixel or per image, and the convolution tiles are chosen from (h, w) alone.
 extern "C" __attribute__((visibility("default"))) int selftok_vae_decode(selftok_vae_t v, const float* z_dev, int B, int h, int w, float* out_dev, int norm_ip,
                                   void* stream) {
   STK_CHECK(v && z_dev && out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_vae_decode: bad argument");
   STK_CHECK(v->finalized, SELFTOK_ERR_STATE, "selftok_vae_finalize has not been called");
   STK_CHECK(v->has_dec, SELFTOK_ERR_MISSING_TENSOR, "selftok_vae_decode: no decoder.* tensors were loaded");
-  STK_CHECK(h == w && (h == 8 || h == 16 || h == 32 || h == 64), SELFTOK_ERR_UNSUPPORTED, "VAE decode: square latents of side 8, 16, 32 or 64");
+  STK_CHECK(h >= 1 && h <= 128 && w >= 1 && w <= 128, SELFTOK_ERR_UNSUPPORTED, "VAE decode: latent sides must be in [1, 128]");
   STK_CUDA(cudaSetDevice(v->device));
   cudaStream_t s = (cudaStream_t)stream;
-  STK_TRY(vae_ensure_ws(v, B, h));
+  STK_TRY(vae_ensure_ws(v, B, h, w));
   VaeCtx c{v, s, B};
   const int ch = v->ch, Cm = ch * v->mult[3];
   int H = h, W = w;
@@ -569,17 +592,20 @@ extern "C" __attribute__((visibility("default"))) int selftok_vae_decode(selftok
   return SELFTOK_OK;
 }
 
-// images_dev [B, 3, H, W] fp32 in [-1, 1] -> the latent distribution's parameters [B, 16, H/8, W/8] fp32 NCHW each (VAE latent
-// space, i.e. BEFORE SD3LatentFormat.process_in): mean_out_dev = `.mode()` (SelftokPipeline.py:215), logvar_out_dev optional.
+// images_dev [B, 3, H, W] fp32 in [-1, 1], H and W multiples of 8 in [8, 1024] -> the latent distribution's parameters
+// [B, 16, H/8, W/8] fp32 NCHW each (VAE latent space, i.e. BEFORE SD3LatentFormat.process_in): mean_out_dev = `.mode()`
+// (SelftokPipeline.py:215), logvar_out_dev optional.  Every downsampled level has even sides (H / 8 may be odd), so the stride-2
+// convolutions keep the polyphase layout.  Batch-invariant as selftok_vae_decode.
 extern "C" __attribute__((visibility("default"))) int selftok_vae_encode(selftok_vae_t v, const float* images_dev, int B, int H, int W, float* mean_out_dev,
                                   float* logvar_out_dev, void* stream) {
   STK_CHECK(v && images_dev && mean_out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_vae_encode: bad argument");
   STK_CHECK(v->finalized, SELFTOK_ERR_STATE, "selftok_vae_finalize has not been called");
   STK_CHECK(v->has_enc, SELFTOK_ERR_MISSING_TENSOR, "selftok_vae_encode: no encoder.* tensors were loaded");
-  STK_CHECK(H == W && (H == 128 || H == 256 || H == 512), SELFTOK_ERR_UNSUPPORTED, "VAE encode: square images of side 128, 256 or 512");
+  STK_CHECK(H % 8 == 0 && W % 8 == 0 && H >= 8 && H <= 1024 && W >= 8 && W <= 1024, SELFTOK_ERR_UNSUPPORTED,
+            "VAE encode: image sides must be multiples of 8 in [8, 1024]");
   STK_CUDA(cudaSetDevice(v->device));
   cudaStream_t s = (cudaStream_t)stream;
-  STK_TRY(vae_ensure_ws(v, B, H / 8));
+  STK_TRY(vae_ensure_ws(v, B, H / 8, W / 8));
   VaeCtx c{v, s, B};
   const int ch = v->ch, Cm = ch * v->mult[3];
   // conv_in: 3 image channels zero-padded to one 64-channel chunk

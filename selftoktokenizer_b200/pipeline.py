@@ -7,8 +7,9 @@ Same constructor signature, attributes and method contracts as the reference cla
     decoding_with_renderer(idx, device)                     -> same, one renderer pass               (:296-322)
 
 Everything between the pixel tensors runs in the CUDA library behind include/selftok_b200.h -- the encoder / VQ / sampler /
-renderer engine and, through `DeviceVAE`, both halves of the SD3 VAE (SURVEY 8f rank 1; diffusers' AutoencoderKL is only the
-source of the VAE weights and the fallback for image sides other than 128 / 256 / 512).  The host keeps what the reference
+renderer engine and, through `DeviceVAE`, both halves of the SD3 VAE (SURVEY 8f rank 1) at every image size the DiT accepts;
+diffusers' AutoencoderKL is only the source of the VAE weights, and the encoder for images above 1024 pixels or with sides that
+are not multiples of 8.  The host keeps what the reference
 keeps on the host: YAML/config, checkpoint loading, the CPU-generator noise draw (:262-264) and numpy<->tensor conversion.
 The latent-boundary methods `encode_latents` / `decode_latents` / `render_latents` are the same calls without the VAE and are
 what the headline of bench.py measures (its `extra.pixel_e2e` record goes through `encoding` / `decoding`).
@@ -80,11 +81,9 @@ class _LatentDist:
 
 class DeviceVAE:
     """`self.vae` with the call shape the pipeline uses (SelftokPipeline.py:215,288,316) on this repo's device VAE (csrc/vae.cu,
-    fp32-faithful split-bf16 GEMMs): `decode` always; `encode` too when the state dict holds the encoder.* half and the images are
-    128 / 256 / 512 pixels square -- otherwise it is delegated to `encoder_vae` (e.g. the diffusers AutoencoderKL).
-    `state_dict`: SDVAE keys, or diffusers keys (`diffusers_keys=True`)."""
-
-    ENCODE_SIDES = (128, 256, 512)
+    fp32-faithful split-bf16 GEMMs): `decode` always; `encode` too when the state dict holds the encoder.* half and the image
+    sides are multiples of 8 in [8, 1024] (selftok_vae_encode's range) -- otherwise it is delegated to `encoder_vae` (e.g. the
+    diffusers AutoencoderKL).  `state_dict`: SDVAE keys, or diffusers keys (`diffusers_keys=True`)."""
 
     def __init__(self, state_dict, device, encoder_vae=None, diffusers_keys: bool = False):
         from .capi import VaeDecoder
@@ -98,12 +97,12 @@ class DeviceVAE:
         return (out,)
 
     def encode(self, x, return_dict=False):
-        if self.has_encoder and x.dim() == 4 and x.shape[2] == x.shape[3] and int(x.shape[2]) in self.ENCODE_SIDES:
+        if self.has_encoder and x.dim() == 4 and all(s % 8 == 0 and 8 <= s <= 1024 for s in x.shape[2:]):
             mean, logvar = self.decoder.encode(x, return_logvar=True)
             return (_LatentDist(mean.to(x.dtype), logvar.to(x.dtype)),)
         if self.encoder_vae is None:
-            raise SelftokError("DeviceVAE.encode: images must be 128/256/512 square with encoder.* weights loaded, or pass "
-                               "encoder_vae=... (e.g. diffusers.AutoencoderKL)")
+            raise SelftokError("DeviceVAE.encode: image sides must be multiples of 8 in [8, 1024] with encoder.* weights loaded, "
+                               "or pass encoder_vae=... (e.g. diffusers.AutoencoderKL)")
         return self.encoder_vae.encode(x, return_dict=return_dict)
 
     def to(self, *a, **k):
@@ -122,7 +121,7 @@ def _load_vae(sd3_path, device, dtype):
     vae = AutoencoderKL.from_pretrained(sd3_path, subfolder="vae")
     vae.to(device).to(dtype)
     vae.eval()
-    # both halves on this repo's device VAE; the diffusers module stays as the fallback for other image sizes
+    # both halves on this repo's device VAE; the diffusers module stays as the encoder outside selftok_vae_encode's range
     return DeviceVAE(vae.state_dict(), device, encoder_vae=vae, diffusers_keys=True)
 
 
