@@ -119,6 +119,23 @@ int selftok_finalize(selftok_handle_t h, void* stream);
 int selftok_export_packed(selftok_handle_t h, const char* path);
 int selftok_import_packed(selftok_handle_t h, const char* path);
 
+/* ---- latent geometry ------------------------------------------------------------------------------------------ */
+/* Latent geometry (lat_h x lat_w, VAE latent pixels) of the following hot-path calls on this handle.  Default and
+ * reset value: cfg.latent x cfg.latent.  Every "latent" shape below means the current geometry: selftok_encode(_host),
+ * selftok_decode(_host), selftok_decode_cfg, the three *_range entries, selftok_decode_step, selftok_dit_velocity and
+ * selftok_workspace_bytes.  Tokens stay [B,K] at every geometry, so ids encoded at one size decode at another.
+ *   - both sides must be positive multiples of dit_patch and of enc_patch (SELFTOK_ERR_BAD_ARG otherwise);
+ *   - at least one positional grid must hold the patch grid: lat / dit_patch <= dit_pos_max or lat / enc_patch <=
+ *     enc_pos_max on both sides (SELFTOK_ERR_UNSUPPORTED otherwise);
+ *   - a renderer handle serves cfg.latent x cfg.latent only (its positional_embedding is [N,D] with a fixed N).
+ * On an error the geometry is unchanged.  Each entry then checks its own grid before any launch and returns
+ * SELFTOK_ERR_UNSUPPORTED beyond it: the encoder's (lat / enc_patch <= enc_pos_max) for encode, the MMDiT's for decode.
+ * The centre crop of each positional grid (the reference's cropped_pos_embed) is built on the calling stream at the first
+ * call of a geometry and kept until selftok_destroy (counted by selftok_device_bytes); CUDA graphs are keyed by geometry, and
+ * the workspaces grow to the largest (batch, geometry) they have to hold.  Mixed geometries inside one call are not
+ * supported. */
+int selftok_set_latent_size(selftok_handle_t h, int lat_h, int lat_w);
+
 /* ---- hot path, device buffers ---------------------------------------------------------------------------- */
 /* x0_dev [B,C,latent,latent] fp32 (VAE latent after SD3LatentFormat.process_in) -> tokens_dev [B,K] int64,
  * outs_q_dev [B,K,code_dim] fp32 (may be NULL), feats_dev [B,K,enc_qdim] fp32 pre-VQ features (may be NULL). */
@@ -227,7 +244,7 @@ int64_t selftok_vae_device_bytes(selftok_vae_t v);
 /* ---- activation workspace.  By default the library allocates ONE device block per operation class (0 = encode,
  * 1 = decode / render / velocity) with cudaMalloc at the first call of a batch size.  A caller that owns device memory
  * (PyTorch's caching allocator) can size it with selftok_workspace_bytes and hand it over with selftok_set_workspace; the
- * library then allocates nothing at call time. */
+ * library then allocates nothing at call time.  selftok_workspace_bytes sizes batch B at the current latent geometry. */
 int64_t selftok_workspace_bytes(selftok_handle_t h, int B, int op);
 int selftok_set_workspace(selftok_handle_t h, int op, void* ws_dev, size_t bytes);
 

@@ -28,7 +28,7 @@ SYMBOLS = [
     "selftok_render_host", "selftok_id_errors", "selftok_workspace_bytes", "selftok_set_workspace", "selftok_last_launch_count", "selftok_device_bytes", "selftok_set_use_graph",
     "selftok_set_profile", "selftok_get_profile", "selftok_k_gemm", "selftok_k_set_gemm_ctas", "selftok_k_ln_mod_f32", "selftok_k_attention_f32",
     "selftok_k_attention_tc", "selftok_decode_range", "selftok_decode_cfg_range", "selftok_render_range", "selftok_k_attention_tc_range",
-    "selftok_decode_step", "selftok_k_quant_e4m3", "selftok_k_ln_mod_e4m3",
+    "selftok_decode_step", "selftok_k_quant_e4m3", "selftok_k_ln_mod_e4m3", "selftok_set_latent_size",
     "selftok_vae_create", "selftok_vae_destroy", "selftok_vae_load_tensor", "selftok_vae_finalize", "selftok_vae_decode", "selftok_vae_encode", "selftok_vae_device_bytes",
 ]
 
@@ -119,6 +119,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.selftok_render_range.argtypes = [vp, vp, vp, i32, vp, vp]
     lib.selftok_k_attention_tc_range.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp]
     lib.selftok_decode_step.argtypes = [vp, vp, vp, vp, vp, vp, i32, vp, vp]
+    lib.selftok_set_latent_size.argtypes = [vp, i32, i32]
     lib.selftok_vae_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.selftok_vae_destroy.argtypes = [vp]
     lib.selftok_vae_load_tensor.argtypes = [vp, C.c_char_p, vp, i32, C.POINTER(i64), i32]
@@ -196,6 +197,7 @@ class Engine:
         h = C.c_void_p()
         check(self.lib.selftok_create(C.byref(cfg), C.byref(h)))
         self.h = h
+        self.latent_hw = (dims.latent, dims.latent)     # geometry of the handle's hot-path calls (selftok_set_latent_size)
         try:
             if not self.restored_from_pack:
                 self._load(state_dict)
@@ -280,12 +282,44 @@ class Engine:
 
     # The C entry points take raw pointers and a batch size only: shapes are checked HERE so that a latent of another
     # resolution (datasize != the engine's geometry) or a short token row fails loudly instead of reading out of bounds.
-    def _check_latent(self, x: torch.Tensor, what: str) -> None:
+    def _check_latent(self, x: torch.Tensor, what: str, latent_hw=None) -> None:
         d = self.dims
-        want = (d.in_channels, d.latent, d.latent)
+        hw = (d.latent, d.latent) if latent_hw is None else latent_hw
+        want = (d.in_channels, *hw)
         if x.dim() != 4 or tuple(x.shape[1:]) != want or x.shape[0] < 1:
+            side = f"(image side {8 * d.latent})" if latent_hw is None else f"(latent_hw={tuple(hw)})"
             raise SelftokError(f"{what}: expected [B, {want[0]}, {want[1]}, {want[2]}] latents for this engine "
-                               f"(image side {8 * d.latent}), got {tuple(x.shape)}")
+                               f"{side}, got {tuple(x.shape)}")
+
+    def set_latent_size(self, lat_h: int, lat_w: int) -> None:
+        """Latent geometry of the following hot-path calls (selftok_set_latent_size).  Tokens stay [B, K] at every size."""
+        check(self.lib.selftok_set_latent_size(self.h, int(lat_h), int(lat_w)))
+        self.latent_hw = (int(lat_h), int(lat_w))
+
+    def _geometry(self, x: torch.Tensor, what: str, latent_hw, encode: bool = False):
+        """-> the latent geometry of a call on x: `latent_hw` (None: the engine's own size), checked against x's shape and the
+        positional grid of the call.  Raises before anything changes; `_set_geometry` switches the handle afterwards."""
+        d = self.dims
+        hw = None
+        if latent_hw is not None:
+            try:
+                hw = (int(latent_hw[0]), int(latent_hw[1]))
+                ok = len(latent_hw) == 2
+            except (TypeError, ValueError, IndexError):
+                ok = False
+            if not ok:
+                raise SelftokError(f"{what}: latent_hw must be a pair (h, w) of ints, got {latent_hw!r}")
+        self._check_latent(x, what, hw)
+        hw = hw or (d.latent, d.latent)
+        p, mx, grid = (d.enc_patch, d.enc_pos_max, "encoder") if encode else (d.dit_patch, d.dit_pos_max, "MMDiT")
+        if max(hw) // p > mx:
+            raise SelftokError(f"{what}: latent {hw[0]} x {hw[1]} is beyond the {grid} positional grid "
+                               f"({mx} x {mx} patches of {p}: latent sides up to {mx * p})")
+        return hw
+
+    def _set_geometry(self, hw) -> None:
+        if hw != self.latent_hw:
+            self.set_latent_size(*hw)
 
     def _check_tokens(self, tokens: torch.Tensor, what: str, batch: Optional[int] = None, is_output: bool = False,
                       ranges: Optional[np.ndarray] = None) -> None:
@@ -316,15 +350,17 @@ class Engine:
             raise SelftokError("selftok_id_errors failed")
         return n
 
-    def encode(self, x0: torch.Tensor, return_aux: bool = False):
-        """x0 [B,C,h,w] fp32 latents -> tokens [B,K] int64 (device)."""
+    def encode(self, x0: torch.Tensor, return_aux: bool = False, *, latent_hw=None):
+        """x0 [B,C,h,w] fp32 latents -> tokens [B,K] int64 (device).  latent_hw=None: (h, w) must be the engine's own size;
+        latent_hw=(h, w): any geometry within the encoder's positional grid, equal to x0's."""
         d = self.dims
-        self._check_latent(x0, "encode")
+        hw = self._geometry(x0, "encode", latent_hw, encode=True)
         x0 = self._dev(x0, torch.float32)
         B = x0.shape[0]
         tokens = torch.empty(B, d.K, dtype=torch.int64, device=self.device)
         outs_q = torch.empty(B, d.K, d.code_dim, dtype=torch.float32, device=self.device) if return_aux else None
         feats = torch.empty(B, d.K, d.enc_qdim, dtype=torch.float32, device=self.device) if return_aux else None
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             check(self.lib.selftok_encode(self.h, x0.data_ptr(), B, tokens.data_ptr(), _ptr(outs_q), _ptr(feats),
                                           _stream_ptr(self.device)))
@@ -359,16 +395,19 @@ class Engine:
             raise SelftokError(f"token_range: expected a (lo, hi) pair or an int array [{B}, 2], got {r.dtype} {r.shape}")
         return np.ascontiguousarray(r, dtype=np.int32)
 
-    def decode(self, tokens: torch.Tensor, noise: torch.Tensor, steps: Optional[int] = None, *, token_range=None) -> torch.Tensor:
+    def decode(self, tokens: torch.Tensor, noise: torch.Tensor, steps: Optional[int] = None, *, token_range=None,
+               latent_hw=None) -> torch.Tensor:
         """tokens [B,K], noise [B,C,h,w] -> latents after `steps` Euler steps.  token_range (see `token_ranges`): image b is decoded
-        from its ids [lo_b, hi_b) only (selftok_decode_range); n generated tokens of the AR order = (K - n, K)."""
-        self._check_latent(noise, "decode (noise)")
+        from its ids [lo_b, hi_b) only (selftok_decode_range); n generated tokens of the AR order = (K - n, K).  latent_hw as in
+        `encode`, within the MMDiT's positional grid."""
+        hw = self._geometry(noise, "decode (noise)", latent_hw)
         rng = None if token_range is None else self.token_ranges(token_range, noise.shape[0])
         self._check_tokens(tokens, "decode", noise.shape[0], ranges=rng)
         tokens = self._dev(tokens, torch.int64)
         noise = self._dev(noise, torch.float32)
         B = tokens.shape[0]
         out = torch.empty_like(noise)
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             if rng is None:
                 check(self.lib.selftok_decode(self.h, tokens.data_ptr(), noise.data_ptr(), B, steps or self.steps,
@@ -379,15 +418,17 @@ class Engine:
         return out
 
     def decode_cfg(self, tokens: torch.Tensor, noise: torch.Tensor, cfg_scale: float, steps: Optional[int] = None, *,
-                   token_range=None) -> torch.Tensor:
+                   token_range=None, latent_hw=None) -> torch.Tensor:
         """Guided sampler: the reference's p_sample_loop(..., uncond_scale=cfg_scale) (rectified_flow.py:280-289).  token_range as
-        in `decode`; every window must keep a visible token at the last executed step (lo <= k of that step)."""
-        self._check_latent(noise, "decode_cfg (noise)")
+        in `decode`; every window must keep a visible token at the last executed step (lo <= k of that step).  latent_hw as in
+        `decode`."""
+        hw = self._geometry(noise, "decode_cfg (noise)", latent_hw)
         rng = None if token_range is None else self.token_ranges(token_range, noise.shape[0])
         self._check_tokens(tokens, "decode_cfg", noise.shape[0], ranges=rng)
         tokens = self._dev(tokens, torch.int64)
         noise = self._dev(noise, torch.float32)
         out = torch.empty_like(noise)
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             if rng is None:
                 check(self.lib.selftok_decode_cfg(self.h, tokens.data_ptr(), noise.data_ptr(), tokens.shape[0], steps or self.steps,
@@ -398,12 +439,13 @@ class Engine:
         return out
 
     def decode_step(self, tokens: torch.Tensor, x: torch.Tensor, step, *, token_range=None, cfg_scale=None,
-                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    out: Optional[torch.Tensor] = None, latent_hw=None) -> torch.Tensor:
         """One Euler step per image at its own schedule row (selftok_decode_step): x [B,C,h,w] -> x - dt[step_b] * v_b.
         `step`: an int for the whole batch or an int array [B].  cfg_scale: None (plain sampler), a float or a float array [B]
         (guided sampler, every image).  token_range as in `decode`.  `out` may be `x` itself.  Running steps 0..n-1 of an image
-        through any sequence of calls, in any batches, is bitwise `decode(steps=n)` / `decode_cfg` of that image alone."""
-        self._check_latent(x, "decode_step (x)")
+        through any sequence of calls, in any batches, is bitwise `decode(steps=n)` / `decode_cfg` of that image alone.  latent_hw as
+        in `decode`: every image of one call has the same size."""
+        hw = self._geometry(x, "decode_step (x)", latent_hw)
         B = x.shape[0]
         rng = None if token_range is None else self.token_ranges(token_range, B)
         st = np.asarray(step)
@@ -434,18 +476,20 @@ class Engine:
             out = torch.empty_like(x)
         elif out.shape != x.shape or out.dtype != torch.float32 or out.device != x.device or not out.is_contiguous():
             raise SelftokError("decode_step: `out` must be a contiguous fp32 device tensor shaped like x")
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             check(self.lib.selftok_decode_step(self.h, tokens.data_ptr(), None if rng is None else rng.ctypes.data, st.ctypes.data,
                                                None if cs is None else cs.ctypes.data, x.data_ptr(), B, out.data_ptr(),
                                                _stream_ptr(self.device)))
         return out
 
-    def dit_velocity(self, tokens: torch.Tensor, x: torch.Tensor, step: int) -> torch.Tensor:
-        self._check_latent(x, "dit_velocity")
+    def dit_velocity(self, tokens: torch.Tensor, x: torch.Tensor, step: int, *, latent_hw=None) -> torch.Tensor:
+        hw = self._geometry(x, "dit_velocity", latent_hw)
         self._check_tokens(tokens, "dit_velocity", x.shape[0])
         tokens = self._dev(tokens, torch.int64)
         x = self._dev(x, torch.float32)
         out = torch.empty_like(x)
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             check(self.lib.selftok_dit_velocity(self.h, tokens.data_ptr(), x.data_ptr(), tokens.shape[0], step,
                                                 out.data_ptr(), _stream_ptr(self.device)))
@@ -467,23 +511,26 @@ class Engine:
         return out
 
     # ------------------------------------------------------------------ hot path (host buffers; copies inside the call)
-    def encode_host(self, x0: torch.Tensor, tokens_out: torch.Tensor) -> torch.Tensor:
+    def encode_host(self, x0: torch.Tensor, tokens_out: torch.Tensor, *, latent_hw=None) -> torch.Tensor:
         if x0.is_cuda or tokens_out.is_cuda or x0.dtype != torch.float32 or tokens_out.dtype != torch.int64 \
                 or not x0.is_contiguous() or not tokens_out.is_contiguous():
             raise SelftokError("encode_host: contiguous host tensors (fp32 latents, int64 tokens) expected")
-        self._check_latent(x0, "encode_host")
+        hw = self._geometry(x0, "encode_host", latent_hw, encode=True)
         self._check_tokens(tokens_out, "encode_host", x0.shape[0], is_output=True)
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             check(self.lib.selftok_encode_host(self.h, x0.data_ptr(), x0.shape[0], tokens_out.data_ptr(), _stream_ptr(self.device)))
         return tokens_out
 
-    def decode_host(self, tokens: torch.Tensor, noise: torch.Tensor, out: torch.Tensor, steps: Optional[int] = None) -> torch.Tensor:
+    def decode_host(self, tokens: torch.Tensor, noise: torch.Tensor, out: torch.Tensor, steps: Optional[int] = None, *,
+                    latent_hw=None) -> torch.Tensor:
         if tokens.is_cuda or noise.is_cuda or out.is_cuda or tokens.dtype != torch.int64 or noise.dtype != torch.float32 \
                 or out.dtype != torch.float32 or not (tokens.is_contiguous() and noise.is_contiguous() and out.is_contiguous()):
             raise SelftokError("decode_host: contiguous host tensors (int64 tokens, fp32 noise / output) expected")
-        self._check_latent(noise, "decode_host (noise)")
-        self._check_latent(out, "decode_host (output)")
+        hw = self._geometry(noise, "decode_host (noise)", latent_hw)
+        self._check_latent(out, "decode_host (output)", hw)
         self._check_tokens(tokens, "decode_host", noise.shape[0])
+        self._set_geometry(hw)
         with torch.cuda.device(self.device):
             check(self.lib.selftok_decode_host(self.h, tokens.data_ptr(), noise.data_ptr(), tokens.shape[0],
                                                steps or self.steps, out.data_ptr(), _stream_ptr(self.device)))
@@ -501,6 +548,7 @@ class Engine:
 
     # ------------------------------------------------------------------ misc
     def workspace_bytes(self, B: int, op: str) -> int:
+        """Bytes of the `op` workspace for batch B at the current geometry (`latent_hw`)."""
         n = int(self.lib.selftok_workspace_bytes(self.h, B, {"encode": 0, "decode": 1}[op]))
         if n < 0:
             raise SelftokError("selftok_workspace_bytes failed")

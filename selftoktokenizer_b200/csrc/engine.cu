@@ -55,8 +55,10 @@ struct Arena {
   }
 };
 
-struct DecodeWs {       // activation workspace of the MMDiT for one batch size
-  int B = 0;
+struct DecodeWs {       // activation workspace of the MMDiT, carved for one batch size and latent geometry
+  int B = 0, lh = 0, lw = 0;
+  char* base = nullptr;                          // the block it is carved from (the caller's or `own`) and its size
+  size_t cap = 0;
   int64_t* tokens = nullptr;
   float *outs_q = nullptr, *x_lat = nullptr, *patch = nullptr, *ctx0 = nullptr, *ctx = nullptr, *x = nullptr;
   float *qkv = nullptr, *o_final = nullptr;      // qkv: fp32 joint buffer (fp32 mode only)
@@ -77,7 +79,9 @@ struct DecodeWs {       // activation workspace of the MMDiT for one batch size
   size_t own_bytes = 0;
 };
 struct EncodeWs {
-  int B = 0;
+  int B = 0, lh = 0, lw = 0;
+  char* base = nullptr;
+  size_t cap = 0;
   float *x0 = nullptr, *patch = nullptr, *x = nullptr, *q = nullptr, *xn = nullptr, *qn = nullptr, *xqkv = nullptr,
         *xkv = nullptr, *qqkv = nullptr, *xattn = nullptr, *qattn = nullptr, *xh = nullptr, *qh = nullptr, *outs_q = nullptr;
   int64_t* tokens = nullptr;
@@ -87,7 +91,9 @@ struct EncodeWs {
 
 struct selftok_engine {
   selftok_config_t cfg;
-  int D = 0, H = 0, Nimg = 0, Nenc = 0;
+  int D = 0, H = 0;
+  // latent geometry of the hot-path calls (selftok_set_latent_size; default cfg.latent x cfg.latent) and its patch counts
+  int lat_h = 0, lat_w = 0, Nimg = 0, Nenc = 0;
   bool finalized = false;
   bool use_graph = true;
   std::unordered_map<std::string, Tensor> w;
@@ -105,19 +111,24 @@ struct selftok_engine {
   float *ctx_mod = nullptr, *x_mod = nullptr, *ctx_last_mod = nullptr, *final_mod = nullptr, *dit_pos = nullptr;
   float *x_mod_u = nullptr, *final_mod_u = nullptr;     // unconditional branch of the guided sampler (optional)
   float* rend_x0 = nullptr;
+  // centre crops of encoder.pos_embed [0] / model.pos_embed [1] for the geometries other than the default one, keyed by the
+  // patch grid (gh, gw); the default crops are enc_pos / dit_pos.  pos_cur: the tables of the current geometry (pos_table)
+  std::map<std::pair<int, int>, float*> pos_crops[2];
+  const float* pos_cur[2] = {nullptr, nullptr};
   bool has_cfg = false;                 // unconditional-branch tables built (selftok_set_cfg_schedule before finalize)
   int* bad_ids = nullptr;               // device counter of out-of-range token ids seen by the lookup kernel
   DecodeWs dws;
   EncodeWs ews;
   void* user_ws[2] = {nullptr, nullptr};          // caller-provided workspaces (selftok_set_workspace): [0] encode, [1] decode / render
   size_t user_ws_bytes[2] = {0, 0};
-  std::map<std::pair<int, int>, std::pair<cudaGraphExec_t, int64_t>> graphs;   // (B, steps) -> (exec, launches)
-  std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, int64_t>> range_graphs;   // token ranges: (B, steps, Lo, Hi)
+  std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, int64_t>> graphs;   // (B, steps, lat_h, lat_w) -> (exec, launches)
+  // token ranges: (B, steps, Lo, Hi, lat_h, lat_w)
+  std::map<std::tuple<int, int, int, int, int, int>, std::pair<cudaGraphExec_t, int64_t>> range_graphs;
   std::vector<int> plan_host;           // token-range plan of the current call, built on the host
   int* plan_pinned = nullptr;           // pinned staging copy of it (an H2D copy from pageable memory would block the host)
   size_t plan_pinned_n = 0;
   cudaEvent_t plan_copied = nullptr;    // recorded after each upload: the staging buffer is reused only once it has completed
-  std::map<int, std::pair<cudaGraphExec_t, int64_t>> enc_graphs;               // encode, B -> (exec, launches)
+  std::map<std::tuple<int, int, int>, std::pair<cudaGraphExec_t, int64_t>> enc_graphs;   // encode, (B, lat_h, lat_w) -> (exec, launches)
   int64_t last_launches = 0;
   // optional per-kernel-class timing (CUDA events around every launch; only meaningful with graphs disabled)
   bool prof_on = false;
@@ -267,6 +278,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_create(const selft
   e->cfg = *cfg;
   e->D = 64 * cfg->dit_depth;
   e->H = cfg->dit_depth;
+  e->lat_h = e->lat_w = cfg->latent;
   e->Nimg = (cfg->latent / cfg->dit_patch) * (cfg->latent / cfg->dit_patch);
   e->Nenc = (cfg->latent / cfg->enc_patch) * (cfg->latent / cfg->enc_patch);
   if (tc_mode(e)) {
@@ -286,9 +298,12 @@ static void free_dws(selftok_engine* e) {
   if (e->dws.own) { cudaFree(e->dws.own); e->bytes -= (int64_t)e->dws.own_bytes; }
   e->dws = DecodeWs();
 }
-static void free_ews(selftok_engine* e) {
-  for (auto& g : e->enc_graphs) cudaGraphExecDestroy(g.second.first);         // graphs hold pointers into the workspace
+static void drop_encode_graphs(selftok_engine* e) {
+  for (auto& g : e->enc_graphs) cudaGraphExecDestroy(g.second.first);
   e->enc_graphs.clear();
+}
+static void free_ews(selftok_engine* e) {
+  drop_encode_graphs(e);                                                      // graphs hold pointers into the workspace
   if (e->ews.own) { cudaFree(e->ews.own); e->bytes -= (int64_t)e->ews.own_bytes; }
   e->ews = EncodeWs();
 }
@@ -401,7 +416,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_finalize(selftok_h
     STK_CHECK(pe->numel == (int64_t)c.enc_pos_max * c.enc_pos_max * c.enc_hidden, SELFTOK_ERR_BAD_ARG, "encoder.pos_embed shape");
     int g = c.latent / c.enc_patch;
     STK_TRY(dalloc(e, e->allocs, &e->enc_pos, (int64_t)g * g * c.enc_hidden));
-    PROF(PC_OTHER, launch_crop_pos(pe->d, e->enc_pos, c.enc_pos_max, g, c.enc_hidden, s));
+    PROF(PC_OTHER, launch_crop_pos(pe->d, e->enc_pos, c.enc_pos_max, g, g, (c.enc_pos_max - g) / 2, (c.enc_pos_max - g) / 2, c.enc_hidden, s));
     GETW(cb, "encoder.quantizer._codebook.embed");
     STK_CHECK(cb->numel == (int64_t)c.codebook_size * c.code_dim, SELFTOK_ERR_BAD_ARG, "codebook shape");
     STK_TRY(dalloc(e, e->allocs, &e->cbt, cb->numel));
@@ -469,7 +484,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_finalize(selftok_h
     STK_CHECK(pe->numel == (int64_t)c.dit_pos_max * c.dit_pos_max * D, SELFTOK_ERR_BAD_ARG, "model.pos_embed shape");
     int g = c.latent / c.dit_patch;
     STK_TRY(dalloc(e, e->allocs, &e->dit_pos, (int64_t)g * g * D));
-    PROF(PC_OTHER, launch_crop_pos(pe->d, e->dit_pos, c.dit_pos_max, g, D, s));
+    PROF(PC_OTHER, launch_crop_pos(pe->d, e->dit_pos, c.dit_pos_max, g, g, (c.dit_pos_max - g) / 2, (c.dit_pos_max - g) / 2, D, s));
   }
   // ---- tensor-core operand planes of the MMDiT linears
   std::vector<std::string> packed_names;
@@ -707,10 +722,12 @@ extern "C" __attribute__((visibility("default"))) int selftok_import_packed(self
 }
 
 // ------------------------------------------------------------------------------------------------ encode
+static int64_t lat_elems(const selftok_engine* e) { return (int64_t)e->cfg.in_channels * e->lat_h * e->lat_w; }   // per image
+
 static int layout_ews(selftok_engine* e, EncodeWs& w, int64_t B, Arena& A) {
   const selftok_config_t& c = e->cfg;
   const int64_t Ni = e->Nenc, K = c.K, Hh = c.enc_hidden, Q = c.enc_qdim;
-  STK_TRY(A.take(&w.x0, B * c.in_channels * c.latent * c.latent));
+  STK_TRY(A.take(&w.x0, B * lat_elems(e)));
   STK_TRY(A.take(&w.patch, B * Ni * c.in_channels * c.enc_patch * c.enc_patch));
   STK_TRY(A.take(&w.x, B * Ni * Hh));
   STK_TRY(A.take(&w.q, B * K * Q));
@@ -727,33 +744,113 @@ static int layout_ews(selftok_engine* e, EncodeWs& w, int64_t B, Arena& A) {
   STK_TRY(A.take(&w.tokens, B * K));
   return 0;
 }
-// carve the workspace of `op` (0 encode, 1 decode / render) for batch B from the caller's block if it is large enough, else from
-// one cudaMalloc of exactly the needed size
-template <typename WS, typename LAYOUT>
-static int place_ws(selftok_engine* e, int op, WS& w, int B, LAYOUT layout) {
+// Carve the workspace of `op` (0 encode, 1 decode / render) for batch B at the current geometry.  The carve is a function of
+// (block, B, geometry) alone, so a graph captured for a (B, geometry) finds its buffers where it left them as long as the block
+// stays.  The block stays while the layout fits in it; otherwise every graph pointing into it is dropped and the layout moves to
+// the caller's block if that is large enough, else to one cudaMalloc of exactly the needed size.
+template <typename WS, typename LAYOUT, typename DROP>
+static int place_ws(selftok_engine* e, int op, WS& w, int B, LAYOUT layout, DROP drop_graphs) {
+  if (w.base && w.B == B && w.lh == e->lat_h && w.lw == e->lat_w) return 0;
   Arena dry;
   dry.dry = true;
   WS scratch;
   STK_TRY(layout(scratch, (int64_t)B, dry));
-  Arena A;
-  if (e->user_ws[op] && e->user_ws_bytes[op] >= dry.off) {
-    A.base = reinterpret_cast<char*>(e->user_ws[op]);
-    A.cap = e->user_ws_bytes[op];
-  } else {
-    STK_CUDA(cudaMalloc(&w.own, dry.off));
-    w.own_bytes = dry.off;
-    e->bytes += (int64_t)dry.off;
-    A.base = reinterpret_cast<char*>(w.own);
-    A.cap = dry.off;
+  if (!w.base || w.cap < dry.off) {
+    drop_graphs();
+    if (w.own) { cudaFree(w.own); e->bytes -= (int64_t)w.own_bytes; }
+    w.own = nullptr; w.own_bytes = 0; w.base = nullptr; w.cap = 0; w.B = 0;
+    if (e->user_ws[op] && e->user_ws_bytes[op] >= dry.off) {
+      w.base = reinterpret_cast<char*>(e->user_ws[op]);
+      w.cap = e->user_ws_bytes[op];
+    } else {
+      STK_CUDA(cudaMalloc(&w.own, dry.off));
+      w.own_bytes = dry.off;
+      e->bytes += (int64_t)dry.off;
+      w.base = reinterpret_cast<char*>(w.own);
+      w.cap = dry.off;
+    }
   }
+  Arena A;
+  A.base = w.base;
+  A.cap = w.cap;
   STK_TRY(layout(w, (int64_t)B, A));
-  w.B = B;
+  w.B = B; w.lh = e->lat_h; w.lw = e->lat_w;
   return 0;
 }
 static int ensure_ews(selftok_engine* e, int B) {
-  if (e->ews.B >= B) return 0;
-  free_ews(e);
-  return place_ws(e, 0, e->ews, B, [&](EncodeWs& w, int64_t b, Arena& A) { return layout_ews(e, w, b, A); });
+  return place_ws(e, 0, e->ews, B, [&](EncodeWs& w, int64_t b, Arena& A) { return layout_ews(e, w, b, A); },
+                  [&] { drop_encode_graphs(e); });
+}
+
+// The patch grid of the current geometry must fit the positional grid of the encoder (enc = true) or the MMDiT.
+static int check_grid(selftok_engine* e, bool enc, const char* who) {
+  const selftok_config_t& c = e->cfg;
+  const int p = enc ? c.enc_patch : c.dit_patch, mx = enc ? c.enc_pos_max : c.dit_pos_max;
+  if (e->lat_h / p > mx || e->lat_w / p > mx) {
+    set_error(std::string(who) + ": latent " + std::to_string(e->lat_h) + " x " + std::to_string(e->lat_w) + " is a " +
+              std::to_string(e->lat_h / p) + " x " + std::to_string(e->lat_w / p) + " patch grid, beyond the " +
+              (enc ? "encoder" : "MMDiT") + " positional grid of " + std::to_string(mx) + " x " + std::to_string(mx) +
+              " (latent sides up to " + std::to_string(mx * p) + ")");
+    return SELFTOK_ERR_UNSUPPORTED;
+  }
+  return 0;
+}
+
+// Points e->pos_cur[enc ? 0 : 1] at the centre crop of the encoder's / MMDiT's positional grid for the current geometry
+// (top = (max - gh) / 2, left = (max - gw) / 2: cropped_pos_embed, models_ours.py:183-202, sd3/mmdit.py:877-896).  The default
+// geometry uses the table built at finalize; any other one is cropped from the full grid once, on the calling stream (so never
+// inside a capture: call this before one), and kept until selftok_destroy.
+static int pos_table(selftok_engine* e, bool enc, cudaStream_t s) {
+  const selftok_config_t& c = e->cfg;
+  const int i = enc ? 0 : 1;
+  if (e->lat_h == c.latent && e->lat_w == c.latent) {
+    e->pos_cur[i] = enc ? e->enc_pos : e->dit_pos;
+    return 0;
+  }
+  STK_TRY(check_grid(e, enc, "positional table"));
+  const int p = enc ? c.enc_patch : c.dit_patch, mx = enc ? c.enc_pos_max : c.dit_pos_max, dim = enc ? c.enc_hidden : e->D;
+  const int gh = e->lat_h / p, gw = e->lat_w / p;
+  auto it = e->pos_crops[i].find(std::make_pair(gh, gw));
+  if (it == e->pos_crops[i].end()) {
+    GETW(pe, enc ? "encoder.pos_embed" : "model.pos_embed");
+    float* t;
+    STK_TRY(dalloc(e, e->allocs, &t, (int64_t)gh * gw * dim));
+    const int64_t l0 = g_launch_count;                      // a one-time table build, not a launch of the call
+    STK_TRY(launch_crop_pos(pe->d, t, mx, gh, gw, (mx - gh) / 2, (mx - gw) / 2, dim, s));
+    g_launch_count = l0;
+    it = e->pos_crops[i].emplace(std::make_pair(gh, gw), t).first;
+  }
+  e->pos_cur[i] = it->second;
+  return 0;
+}
+
+extern "C" __attribute__((visibility("default"))) int selftok_set_latent_size(selftok_handle_t e, int lat_h, int lat_w) {
+  STK_CHECK(e, SELFTOK_ERR_BAD_ARG, "null handle");
+  const selftok_config_t& c = e->cfg;
+  const std::string hw = std::to_string(lat_h) + " x " + std::to_string(lat_w);
+  if (lat_h <= 0 || lat_w <= 0 || lat_h % c.dit_patch || lat_w % c.dit_patch || lat_h % c.enc_patch || lat_w % c.enc_patch) {
+    set_error("selftok_set_latent_size: latent " + hw + ": both sides must be positive multiples of dit_patch (" +
+              std::to_string(c.dit_patch) + ") and enc_patch (" + std::to_string(c.enc_patch) + ")");
+    return SELFTOK_ERR_BAD_ARG;
+  }
+  const bool dit_ok = lat_h / c.dit_patch <= c.dit_pos_max && lat_w / c.dit_patch <= c.dit_pos_max;
+  const bool enc_ok = lat_h / c.enc_patch <= c.enc_pos_max && lat_w / c.enc_patch <= c.enc_pos_max;
+  if (!dit_ok && !enc_ok) {
+    set_error("selftok_set_latent_size: latent " + hw + " is beyond both positional grids (latent sides up to " +
+              std::to_string(c.dit_pos_max * c.dit_patch) + " for decode, " + std::to_string(c.enc_pos_max * c.enc_patch) +
+              " for encode)");
+    return SELFTOK_ERR_UNSUPPORTED;
+  }
+  if (c.renderer && (lat_h != c.latent || lat_w != c.latent)) {
+    set_error("selftok_set_latent_size: a renderer handle serves " + std::to_string(c.latent) + " x " + std::to_string(c.latent) +
+              " latents only (model.positional_embedding has a fixed number of rows), got " + hw);
+    return SELFTOK_ERR_UNSUPPORTED;
+  }
+  e->lat_h = lat_h;
+  e->lat_w = lat_w;
+  e->Nimg = (lat_h / c.dit_patch) * (lat_w / c.dit_patch);
+  e->Nenc = (lat_h / c.enc_patch) * (lat_w / c.enc_patch);
+  return SELFTOK_OK;
 }
 
 // Encoder.forward up to the quantizer input (models_ours.py:204-219,315-343; modules.py:310-327)
@@ -763,10 +860,10 @@ static int encoder_features(selftok_engine* e, const float* x0, int B, cudaStrea
   const int Ni = e->Nenc, K = c.K, Hh = c.enc_hidden, Q = c.enc_qdim;
   const int64_t Mx = (int64_t)B * Ni, Mq = (int64_t)B * K;
   const float eps = 1e-6f;
-  PROF(PC_OTHER, launch_patchify(x0, w.patch, B, c.in_channels, c.latent, c.latent, c.enc_patch, s));
+  PROF(PC_OTHER, launch_patchify(x0, w.patch, B, c.in_channels, e->lat_h, e->lat_w, c.enc_patch, s));
   {
     Epilogue ep;
-    ep.out = w.x; ep.addtab = e->enc_pos; ep.add_ld = Hh; ep.add_period = Ni;
+    ep.out = w.x; ep.addtab = e->pos_cur[0]; ep.add_ld = Hh; ep.add_period = Ni;
     STK_TRY(lin32(e, "encoder.x_embedder.proj", w.patch, c.in_channels * c.enc_patch * c.enc_patch, Mx, ep, s));
     GETW(qt, "encoder.query_tokens");
     STK_CHECK(qt->numel == (int64_t)K * Q, SELFTOK_ERR_BAD_ARG, "query_tokens shape");
@@ -834,7 +931,9 @@ extern "C" __attribute__((visibility("default"))) int selftok_encode(selftok_han
                               float* feats_dev, void* stream) {
   HOT_PROLOGUE(e);
   STK_CHECK(x0_dev && tokens_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_encode: bad argument");
+  STK_TRY(check_grid(e, true, "selftok_encode"));
   STK_TRY(ensure_ews(e, B));
+  STK_TRY(pos_table(e, true, s));
   const int64_t R = (int64_t)B * e->cfg.K;
   EncodeWs& w = e->ews;
   if (!e->use_graph || e->prof_on) {                       // eager (per-launch profiling needs real launches)
@@ -844,9 +943,10 @@ extern "C" __attribute__((visibility("default"))) int selftok_encode(selftok_han
   } else {
     // one CUDA graph per batch size over the workspace's own input / output buffers (the ~250 launches of the 16 dual blocks
     // dominate a small-batch encode when issued one by one); the caller's buffers are copied in and out around the replay
-    const int64_t nlat = (int64_t)B * e->cfg.in_channels * e->cfg.latent * e->cfg.latent;
+    const int64_t nlat = (int64_t)B * lat_elems(e);
     if (x0_dev != w.x0) STK_CUDA(cudaMemcpyAsync(w.x0, x0_dev, sizeof(float) * nlat, cudaMemcpyDeviceToDevice, s));
-    auto it = e->enc_graphs.find(B);
+    const auto key = std::make_tuple(B, e->lat_h, e->lat_w);
+    auto it = e->enc_graphs.find(key);
     if (it == e->enc_graphs.end()) {
       cudaStream_t cs;
       STK_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
@@ -868,7 +968,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_encode(selftok_han
       cudaGraphExec_t exec;
       STK_CUDA(cudaGraphInstantiate(&exec, graph, 0));
       cudaGraphDestroy(graph);
-      it = e->enc_graphs.emplace(B, std::make_pair(exec, g_launch_count - l0)).first;
+      it = e->enc_graphs.emplace(key, std::make_pair(exec, g_launch_count - l0)).first;
     }
     STK_CUDA(cudaGraphLaunch(it->second.first, s));
     e->last_launches = it->second.second;
@@ -950,7 +1050,7 @@ static int layout_dws(selftok_engine* e, DecodeWs& w, int64_t B, Arena& A) {
   const int64_t K = c.K, N = e->Nimg, D = e->D, S = K + N;
   STK_TRY(A.take(&w.tokens, B * K));
   STK_TRY(A.take(&w.outs_q, B * K * c.code_dim));
-  STK_TRY(A.take(&w.x_lat, B * c.in_channels * c.latent * c.latent));
+  STK_TRY(A.take(&w.x_lat, B * lat_elems(e)));
   STK_TRY(A.take(&w.patch, B * N * c.in_channels * c.dit_patch * c.dit_patch));
   STK_TRY(A.take(&w.ctx0, B * K * D));
   STK_TRY(A.take(&w.ctx, B * K * D));
@@ -1003,10 +1103,8 @@ static void drop_decode_graphs(selftok_engine* e) {
   e->range_graphs.clear();
 }
 static int ensure_dws(selftok_engine* e, int B) {
-  if (e->dws.B >= B) return 0;
-  drop_decode_graphs(e);                                            // graphs hold pointers into the old workspace
-  free_dws(e);
-  return place_ws(e, 1, e->dws, B, [&](DecodeWs& w, int64_t b, Arena& A) { return layout_dws(e, w, b, A); });
+  return place_ws(e, 1, e->dws, B, [&](DecodeWs& w, int64_t b, Arena& A) { return layout_dws(e, w, b, A); },
+                  [&] { drop_decode_graphs(e); });
 }
 
 // One stream of one JointBlock: LN+modulate -> qkv GEMM into the joint buffer   (mmdit.py:441-483, 521-529)
@@ -1061,7 +1159,7 @@ static int x_embed(selftok_engine* e, int B, cudaStream_t s) {
   DecodeWs& w = e->dws;
   const int D = e->D, N = e->Nimg, Kp = c.in_channels * c.dit_patch * c.dit_patch;
   Epilogue ep;
-  ep.out = w.x; ep.addtab = e->dit_pos; ep.add_ld = D; ep.add_period = N;
+  ep.out = w.x; ep.addtab = e->pos_cur[1]; ep.add_ld = D; ep.add_period = N;
   if (!tc_mode(e) || Kp % 8 != 0) return lin32(e, "model.x_embedder.proj", w.patch, Kp, (int64_t)B * N, ep, s);
   PROF(PC_OTHER, launch_split_bf16(w.patch, w.patch_hi, w.patch_lo, (int64_t)B * N * Kp, s, 0));
   GETW(Bv, "model.x_embedder.proj.bias");
@@ -1255,7 +1353,7 @@ static int dit_forward(selftok_engine* e, int B, int step, cudaStream_t s, const
   int Kc, Lo;
   const int* plan;
   window_step(win, B, step, e->k[step] + 1, &Kc, &plan, &Lo);
-  PROF(PC_OTHER, launch_patchify(w.x_lat, w.patch, B, c.in_channels, c.latent, c.latent, c.dit_patch, s));
+  PROF(PC_OTHER, launch_patchify(w.x_lat, w.patch, B, c.in_channels, e->lat_h, e->lat_w, c.dit_patch, s));
   STK_TRY(x_embed(e, B, s));
   if (Kc > 0) PROF(PC_OTHER, launch_copy_rows(w.ctx0 + (int64_t)Lo * D, (int64_t)c.K * D, w.ctx, (int64_t)Kc * D, B, (int64_t)Kc * D, s));
   // context rows see the image keys unless the handle was created with context_see_xt = 0 (sd3/mmdit.py:1012,1060; the
@@ -1276,7 +1374,7 @@ static int dit_forward_cfg(selftok_engine* e, int B, int step, cudaStream_t s, c
   window_step(win, B, step, e->k[step] + 1, &Kc, &plan, &Lo);
   STK_CHECK(e->has_cfg, SELFTOK_ERR_STATE, "guided sampling needs selftok_set_cfg_schedule before selftok_finalize");
   STK_CHECK(Kc > 0, SELFTOK_ERR_BAD_ARG, "guided sampling needs a visible context token at every step");
-  PROF(PC_OTHER, launch_patchify(w.x_lat, w.patch, B, c.in_channels, c.latent, c.latent, c.dit_patch, s));
+  PROF(PC_OTHER, launch_patchify(w.x_lat, w.patch, B, c.in_channels, e->lat_h, e->lat_w, c.dit_patch, s));
   STK_TRY(x_embed(e, B, s));
   PROF(PC_OTHER, launch_copy_rows(w.ctx0 + (int64_t)Lo * D, (int64_t)c.K * D, w.ctx, (int64_t)Kc * D, B, (int64_t)Kc * D, s));
   STK_TRY(joint_blocks(e, B, Kc, step, /*ctx_self=*/true, s, /*uncond=*/false, w.o_final, plan, Lo));
@@ -1294,11 +1392,12 @@ static int decode_body(selftok_engine* e, int B, int steps, cudaStream_t s, bool
     // euler_step (rectified_flow.py:301-303): x <- x - (t_i - t_{i+1}) * v, fused with unpatchify
     if (!guided) {
       STK_TRY(dit_forward(e, B, i, s, win));
-      PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, w.x_lat, w.x_lat, e->dt[i], B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s));
+      PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, w.x_lat, w.x_lat, e->dt[i], B, c.in_channels, e->lat_h / c.dit_patch,
+                                            e->lat_w / c.dit_patch, c.dit_patch, s));
     } else {
       STK_TRY(dit_forward_cfg(e, B, i, s, win));
-      PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, w.x_lat, w.x_lat, e->dt[i], B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s,
-                                            w.o_final_u, cfg_scale));
+      PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, w.x_lat, w.x_lat, e->dt[i], B, c.in_channels, e->lat_h / c.dit_patch,
+                                            e->lat_w / c.dit_patch, c.dit_patch, s, w.o_final_u, cfg_scale));
     }
   }
   return 0;
@@ -1443,13 +1542,15 @@ static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const floa
   STK_CHECK(tokens_dev && noise_dev && x0_out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_decode: bad argument");
   STK_CHECK(!e->cfg.renderer, SELFTOK_ERR_STATE, "handle was created for the renderer; use selftok_render");
   STK_CHECK(steps > 0 && steps <= e->steps, SELFTOK_ERR_BAD_ARG, "steps exceeds the schedule");
+  STK_TRY(check_grid(e, false, guided ? "selftok_decode_cfg" : "selftok_decode"));
   Window win;
   if (range_host) STK_TRY(plan_window(e, range_host, B, steps, false, guided, &win));
   STK_TRY(ensure_dws(e, B));
+  STK_TRY(pos_table(e, false, s));
   DecodeWs& w = e->dws;
   if (range_host) STK_TRY(upload_window(e, &win, B, s));
   const Window* wp = range_host ? &win : nullptr;
-  const int64_t nlat = (int64_t)B * e->cfg.in_channels * e->cfg.latent * e->cfg.latent;
+  const int64_t nlat = (int64_t)B * lat_elems(e);
   if (tokens_dev != w.tokens) STK_CUDA(cudaMemcpyAsync(w.tokens, tokens_dev, sizeof(int64_t) * B * e->cfg.K, cudaMemcpyDeviceToDevice, s));
   if (noise_dev != w.x_lat) STK_CUDA(cudaMemcpyAsync(w.x_lat, noise_dev, sizeof(float) * nlat, cudaMemcpyDeviceToDevice, s));
   // eager when asked to, for the guided loop (cfg_scale is a kernel argument) and whenever per-launch profiling is on (events
@@ -1460,13 +1561,14 @@ static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const floa
   } else {
     // token-range calls have their own graphs, keyed by the rounded window bounds: the plan itself is read at run time, so one
     // graph serves every range set with the same (Lo, Hi)
-    const auto rkey = std::make_tuple(B, steps, win.Lo, win.Hi);
+    const auto rkey = std::make_tuple(B, steps, win.Lo, win.Hi, e->lat_h, e->lat_w);
+    const auto dkey = std::make_tuple(B, steps, e->lat_h, e->lat_w);
     std::pair<cudaGraphExec_t, int64_t>* g = nullptr;
     if (wp) {
       auto f = e->range_graphs.find(rkey);
       if (f != e->range_graphs.end()) g = &f->second;
     } else {
-      auto f = e->graphs.find(std::make_pair(B, steps));
+      auto f = e->graphs.find(dkey);
       if (f != e->graphs.end()) g = &f->second;
     }
     if (!g) {
@@ -1490,7 +1592,7 @@ static int decode_impl(selftok_handle_t e, const int64_t* tokens_dev, const floa
       STK_CUDA(cudaGraphInstantiate(&exec, graph, 0));
       cudaGraphDestroy(graph);
       const auto val = std::make_pair(exec, g_launch_count - l0);
-      g = wp ? &e->range_graphs.emplace(rkey, val).first->second : &e->graphs.emplace(std::make_pair(B, steps), val).first->second;
+      g = wp ? &e->range_graphs.emplace(rkey, val).first->second : &e->graphs.emplace(dkey, val).first->second;
     }
     STK_CUDA(cudaGraphLaunch(g->first, s));
     e->last_launches = g->second;
@@ -1509,6 +1611,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_decode_step(selfto
   STK_CHECK(!e->cfg.renderer, SELFTOK_ERR_STATE, "selftok_decode_step: handle was created for the renderer");
   const bool guided = cfg_scale_host != nullptr;
   STK_CHECK(!guided || e->has_cfg, SELFTOK_ERR_STATE, "selftok_decode_step: guided steps need selftok_set_cfg_schedule before finalize");
+  STK_TRY(check_grid(e, false, "selftok_decode_step"));
   const selftok_config_t& c = e->cfg;
   const int K = c.K, N = e->Nimg;
   // the per-image block, validated before anything is launched
@@ -1542,6 +1645,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_decode_step(selfto
     cmax = cb > cmax ? cb : cmax;
   }
   STK_TRY(ensure_dws(e, B));
+  STK_TRY(pos_table(e, false, s));
   DecodeWs& w = e->dws;
   STK_TRY(upload_plan(e, w.pk, s));
   int* rows = w.pk + (int64_t)PK_IMG_INTS * B;
@@ -1564,7 +1668,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_decode_step(selfto
     ep.out = w.ctx; ep.addtab = cp->d; ep.add_ld = e->D; ep.tab_rows = pk.ctx_pos;
     STK_TRY(lin32(e, "model.context_embedder", w.outs_q, c.code_dim, Mc, ep, s));
   }
-  PROF(PC_OTHER, launch_patchify(x_dev, w.patch, B, c.in_channels, c.latent, c.latent, c.dit_patch, s));
+  PROF(PC_OTHER, launch_patchify(x_dev, w.patch, B, c.in_channels, e->lat_h, e->lat_w, c.dit_patch, s));
   STK_TRY(x_embed(e, B, s));
   if (!guided) {
     STK_TRY(joint_blocks(e, B, 0, 0, /*ctx_self=*/c.context_see_xt == 0, s, false, w.o_final, nullptr, 0, &pk));
@@ -1576,8 +1680,8 @@ extern "C" __attribute__((visibility("default"))) int selftok_decode_step(selfto
     pu.Mc = 0; pu.S = N;
     STK_TRY(joint_blocks(e, B, 0, 0, /*ctx_self=*/false, s, /*uncond=*/true, w.o_final_u, nullptr, 0, &pu));
   }
-  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, x_dev, x_out_dev, 0.f, B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s,
-                                        guided ? w.o_final_u : nullptr, 1.f, pk.dt, guided ? pk.scale : nullptr));
+  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, x_dev, x_out_dev, 0.f, B, c.in_channels, e->lat_h / c.dit_patch, e->lat_w / c.dit_patch,
+                                        c.dit_patch, s, guided ? w.o_final_u : nullptr, 1.f, pk.dt, guided ? pk.scale : nullptr));
   e->last_launches = g_launch_count - launches0;
   return SELFTOK_OK;
 }
@@ -1588,16 +1692,19 @@ extern "C" __attribute__((visibility("default"))) int selftok_dit_velocity(selft
   STK_CHECK(tokens_dev && x_dev && v_out_dev && B > 0, SELFTOK_ERR_BAD_ARG, "selftok_dit_velocity: bad argument");
   STK_CHECK(!e->cfg.renderer, SELFTOK_ERR_STATE, "renderer handle");
   STK_CHECK(step >= 0 && step < e->steps, SELFTOK_ERR_BAD_ARG, "step out of range");
+  STK_TRY(check_grid(e, false, "selftok_dit_velocity"));
   STK_TRY(ensure_dws(e, B));
+  STK_TRY(pos_table(e, false, s));
   DecodeWs& w = e->dws;
   const selftok_config_t& c = e->cfg;
-  const int64_t nlat = (int64_t)B * c.in_channels * c.latent * c.latent;
+  const int64_t nlat = (int64_t)B * lat_elems(e);
   STK_CUDA(cudaMemcpyAsync(w.tokens, tokens_dev, sizeof(int64_t) * B * c.K, cudaMemcpyDeviceToDevice, s));
   STK_CUDA(cudaMemcpyAsync(w.x_lat, x_dev, sizeof(float) * nlat, cudaMemcpyDeviceToDevice, s));
   STK_TRY(run_lookup(e, w.tokens, B, w.outs_q, s));
   STK_TRY(context_embed(e, B, s));
   STK_TRY(dit_forward(e, B, step, s));
-  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, nullptr, v_out_dev, -1.f, B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s));
+  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, nullptr, v_out_dev, -1.f, B, c.in_channels, e->lat_h / c.dit_patch,
+                                        e->lat_w / c.dit_patch, c.dit_patch, s));
   e->last_launches = g_launch_count - launches0;
   return SELFTOK_OK;
 }
@@ -1621,7 +1728,8 @@ static int render_impl(selftok_handle_t e, const int64_t* tokens_dev, int B, flo
   PROF(PC_OTHER, launch_bcast_rows(e->rend_x0, nullptr, w.x, B, e->Nimg, e->D, s));
   PROF(PC_OTHER, launch_copy_rows(w.ctx0 + (int64_t)Lo * e->D, (int64_t)c.K * e->D, w.ctx, (int64_t)Kc * e->D, B, (int64_t)Kc * e->D, s));
   STK_TRY(joint_blocks(e, B, Kc, 0, /*ctx_self=*/true, s, false, nullptr, range_host ? win.plan : nullptr, Lo));
-  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, nullptr, x0_out_dev, -1.f, B, c.in_channels, c.latent / c.dit_patch, c.dit_patch, s));
+  PROF(PC_OTHER, launch_unpatchify_axpy(w.o_final, nullptr, x0_out_dev, -1.f, B, c.in_channels, e->lat_h / c.dit_patch,
+                                        e->lat_w / c.dit_patch, c.dit_patch, s));
   e->last_launches = g_launch_count - launches0;
   return SELFTOK_OK;
 }
@@ -1641,8 +1749,9 @@ extern "C" __attribute__((visibility("default"))) int selftok_encode_host(selfto
   STK_CHECK(e->finalized, SELFTOK_ERR_STATE, "selftok_finalize has not been called");
   STK_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
+  STK_TRY(check_grid(e, true, "selftok_encode_host"));
   STK_TRY(ensure_ews(e, B));
-  const int64_t nlat = (int64_t)B * e->cfg.in_channels * e->cfg.latent * e->cfg.latent;
+  const int64_t nlat = (int64_t)B * lat_elems(e);
   STK_CUDA(cudaMemcpyAsync(e->ews.x0, x0_host, sizeof(float) * nlat, cudaMemcpyHostToDevice, s));
   STK_TRY(selftok_encode(e, e->ews.x0, B, e->ews.tokens, nullptr, nullptr, stream));
   STK_CUDA(cudaMemcpyAsync(tokens_host, e->ews.tokens, sizeof(int64_t) * B * e->cfg.K, cudaMemcpyDeviceToHost, s));
@@ -1656,9 +1765,10 @@ extern "C" __attribute__((visibility("default"))) int selftok_decode_host(selfto
   STK_CHECK(e->finalized, SELFTOK_ERR_STATE, "selftok_finalize has not been called");
   STK_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
+  STK_TRY(check_grid(e, false, "selftok_decode_host"));
   STK_TRY(ensure_dws(e, B));
   DecodeWs& w = e->dws;
-  const int64_t nlat = (int64_t)B * e->cfg.in_channels * e->cfg.latent * e->cfg.latent;
+  const int64_t nlat = (int64_t)B * lat_elems(e);
   STK_CUDA(cudaMemcpyAsync(w.tokens, tokens_host, sizeof(int64_t) * B * e->cfg.K, cudaMemcpyHostToDevice, s));
   STK_CUDA(cudaMemcpyAsync(w.x_lat, noise_host, sizeof(float) * nlat, cudaMemcpyHostToDevice, s));
   STK_TRY(selftok_decode(e, w.tokens, w.x_lat, B, steps, w.x_lat, stream));
@@ -1674,7 +1784,7 @@ extern "C" __attribute__((visibility("default"))) int selftok_render_host(selfto
   cudaStream_t s = (cudaStream_t)stream;
   STK_TRY(ensure_dws(e, B));
   DecodeWs& w = e->dws;
-  const int64_t nlat = (int64_t)B * e->cfg.in_channels * e->cfg.latent * e->cfg.latent;
+  const int64_t nlat = (int64_t)B * lat_elems(e);
   STK_CUDA(cudaMemcpyAsync(w.tokens, tokens_host, sizeof(int64_t) * B * e->cfg.K, cudaMemcpyHostToDevice, s));
   STK_TRY(selftok_render(e, w.tokens, B, w.x_lat, stream));
   STK_CUDA(cudaMemcpyAsync(x0_out_host, w.x_lat, sizeof(float) * nlat, cudaMemcpyDeviceToHost, s));

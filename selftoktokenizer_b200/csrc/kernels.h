@@ -137,10 +137,10 @@ int launch_lookup_ln3(const int64_t* ids, int64_t R, const float* codebook, int 
                       const int* range = nullptr, int K = 0, const int* gather = nullptr);
 // [B,C,Hh,Ww] latents -> [B*(Hh/p)*(Ww/p), C*p*p] patch rows ((c,ph,pw) fastest-last, Conv2d weight order)
 int launch_patchify(const float* x, float* out, int B, int C, int Hh, int Ww, int p, cudaStream_t s);
-// x_lat[b,c,h*p+ph,w*p+pw] = x_in[...] - dt * o[b, h*g+w, (ph*p+pw)*C + c]   (unpatchify + Euler; dt = -1 & x_in NULL: plain unpatchify)
-// o_u != NULL (guided sampler): v = o_u + cfg_scale * (o - o_u) first.  dt_img / scale_img != NULL: device [B] per-image dt and
-// cfg_scale instead of the scalars
-int launch_unpatchify_axpy(const float* o, const float* x_in, float* x_out, float dt, int B, int C, int g, int p,
+// x_lat[b,c,h*p+ph,w*p+pw] = x_in[...] - dt * o[b, h*gw+w, (ph*p+pw)*C + c]   (unpatchify of a gh x gw patch grid + Euler; dt = -1
+// & x_in NULL: plain unpatchify).  o_u != NULL (guided sampler): v = o_u + cfg_scale * (o - o_u) first.  dt_img / scale_img != NULL:
+// device [B] per-image dt and cfg_scale instead of the scalars
+int launch_unpatchify_axpy(const float* o, const float* x_in, float* x_out, float dt, int B, int C, int gh, int gw, int p,
                            cudaStream_t s, const float* o_u = nullptr, float cfg_scale = 1.f, const float* dt_img = nullptr,
                            const float* scale_img = nullptr);
 // Per-row maps of a packed step call from its per-image block blk = [B][2] (off_b, c_b) | [B] lo_b | [B] step_b: context row
@@ -156,8 +156,8 @@ int launch_transpose(const float* in, float* out, int rows, int cols, cudaStream
 int launch_split_bf16(const float* in, __nv_bfloat16* hi, __nv_bfloat16* lo, int64_t n, cudaStream_t s, int fp16 = 0);
 // out[b, r, :] = src[r, :] for b in 0..B-1 (broadcast rows), optionally + add[r,:]
 int launch_bcast_rows(const float* src, const float* add, float* out, int B, int64_t rows, int64_t cols, cudaStream_t s);
-// centre crop of a [max,max,D] positional grid to [g,g,D]
-int launch_crop_pos(const float* pos, float* out, int max_size, int g, int D, cudaStream_t s);
+// window [top, top + gh) x [left, left + gw) of a [max,max,D] positional grid -> [gh,gw,D]
+int launch_crop_pos(const float* pos, float* out, int max_size, int gh, int gw, int top, int left, int D, cudaStream_t s);
 int launch_copy_rows(const float* src, int64_t src_bs, float* dst, int64_t dst_bs, int B, int64_t n_per_batch, cudaStream_t s);
 
 // ---- wgmma GEMM (gemm_tc.cu) ----------------------------------------------------------------------------------

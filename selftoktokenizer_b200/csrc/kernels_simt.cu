@@ -1033,27 +1033,27 @@ int launch_patchify(const float* x, float* out, int B, int C, int Hh, int Ww, in
 // x_prev = x - (a_t - a_prev) * v (sd3/rectified_flow.py:303).
 // Guided sampler (rectified_flow.py:280-289): with o_u the velocity is  v = v_u + cfg_scale * (v_c - v_u)  before the update.
 __global__ void unpatchify_axpy_kernel(const float* __restrict__ o, const float* __restrict__ x_in, float* __restrict__ x_out,
-                                       float dt, int B, int C, int g, int p, const float* __restrict__ o_u, float cfg_scale,
+                                       float dt, int B, int C, int gh, int gw, int p, const float* __restrict__ o_u, float cfg_scale,
                                        const float* __restrict__ dt_img, const float* __restrict__ scale_img) {
-  const int Hh = g * p;
-  const int64_t total = (int64_t)B * C * Hh * Hh;
+  const int Hh = gh * p, Ww = gw * p;
+  const int64_t total = (int64_t)B * C * Hh * Ww;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int xw = (int)(i % Hh); int64_t t = i / Hh;
+    int xw = (int)(i % Ww); int64_t t = i / Ww;
     int yh = (int)(t % Hh); t /= Hh; int c = (int)(t % C); int b = (int)(t / C);
     int h = yh / p, ph = yh % p, w = xw / p, pw = xw % p;
-    const int64_t oi = ((int64_t)b * g * g + h * g + w) * (p * p * C) + (ph * p + pw) * C + c;
+    const int64_t oi = ((int64_t)b * gh * gw + h * gw + w) * (p * p * C) + (ph * p + pw) * C + c;
     const float dtb = dt_img ? dt_img[b] : dt, csb = scale_img ? scale_img[b] : cfg_scale;
     float v = o[oi];
     if (o_u) { const float vu = o_u[oi]; v = vu + csb * (v - vu); }
     x_out[i] = x_in ? (x_in[i] - dtb * v) : v;
   }
 }
-int launch_unpatchify_axpy(const float* o, const float* x_in, float* x_out, float dt, int B, int C, int g, int p,
+int launch_unpatchify_axpy(const float* o, const float* x_in, float* x_out, float dt, int B, int C, int gh, int gw, int p,
                            cudaStream_t s, const float* o_u, float cfg_scale, const float* dt_img, const float* scale_img) {
-  STK_CHECK(o && x_out, -1, "unpatchify: bad arguments");
-  int64_t total = (int64_t)B * C * g * p * g * p;
-  unpatchify_axpy_kernel<<<(unsigned)((total + 255) / 256 > 4096 ? 4096 : (total + 255) / 256), 256, 0, s>>>(o, x_in, x_out, dt, B, C, g, p, o_u, cfg_scale,
-                                                                                                           dt_img, scale_img);
+  STK_CHECK(o && x_out && gh > 0 && gw > 0, -1, "unpatchify: bad arguments");
+  int64_t total = (int64_t)B * C * gh * p * gw * p;
+  unpatchify_axpy_kernel<<<(unsigned)((total + 255) / 256 > 4096 ? 4096 : (total + 255) / 256), 256, 0, s>>>(o, x_in, x_out, dt, B, C, gh, gw, p,
+                                                                                                           o_u, cfg_scale, dt_img, scale_img);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;
@@ -1185,17 +1185,19 @@ int launch_bcast_rows(const float* src, const float* add, float* out, int B, int
   return 0;
 }
 
-__global__ void crop_pos_kernel(const float* __restrict__ pos, float* __restrict__ out, int max_size, int g, int D) {
-  const int top = (max_size - g) / 2, left = (max_size - g) / 2;
-  const int64_t total = (int64_t)g * g * D;
+__global__ void crop_pos_kernel(const float* __restrict__ pos, float* __restrict__ out, int max_size, int gh, int gw, int top,
+                                int left, int D) {
+  const int64_t total = (int64_t)gh * gw * D;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int d = (int)(i % D); int64_t t = i / D; int w = (int)(t % g), h = (int)(t / g);
+    int d = (int)(i % D); int64_t t = i / D; int w = (int)(t % gw), h = (int)(t / gw);
     out[i] = pos[((int64_t)(top + h) * max_size + left + w) * D + d];
   }
 }
-int launch_crop_pos(const float* pos, float* out, int max_size, int g, int D, cudaStream_t s) {
-  int64_t total = (int64_t)g * g * D;
-  crop_pos_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(pos, out, max_size, g, D);
+int launch_crop_pos(const float* pos, float* out, int max_size, int gh, int gw, int top, int left, int D, cudaStream_t s) {
+  STK_CHECK(pos && out && gh > 0 && gw > 0 && top >= 0 && left >= 0 && top + gh <= max_size && left + gw <= max_size, -1,
+            "crop_pos: the window leaves the grid");
+  int64_t total = (int64_t)gh * gw * D;
+  crop_pos_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(pos, out, max_size, gh, gw, top, left, D);
   count_launch();
   STK_CUDA(cudaGetLastError());
   return 0;

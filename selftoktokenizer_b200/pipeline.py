@@ -20,8 +20,9 @@ buffers are not incremented; no host syncs inside the loop.
 """
 from __future__ import annotations
 
+import math
 import os
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
@@ -123,6 +124,23 @@ def _load_vae(sd3_path, device, dtype):
     vae.eval()
     # both halves on this repo's device VAE; the diffusers module stays as the encoder outside selftok_vae_encode's range
     return DeviceVAE(vae.state_dict(), device, encoder_vae=vae, diffusers_keys=True)
+
+
+def latent_size(size, dims: SelftokDims, encode: bool = False) -> Tuple[int, int]:
+    """Pixel size -- an int or (H, W) -- -> the latent geometry (H // 8, W // 8) one engine serves it at.  Both sides must be
+    multiples of 8 x the patch size (16 for the shipped configs) and the patch grid must fit the encoder's (encode=True) or the
+    MMDiT's positional grid, as the reference's cropped_pos_embed requires (models_ours.py:183-202, sd3/mmdit.py:877-896)."""
+    hw = (size, size) if isinstance(size, (int, np.integer)) else tuple(size)
+    if len(hw) != 2 or not all(isinstance(v, (int, np.integer)) for v in hw):
+        raise SelftokError(f"size must be an int or a pair (H, W) of ints, got {size!r}")
+    H, W = int(hw[0]), int(hw[1])
+    unit = 8 * math.lcm(dims.dit_patch, dims.enc_patch)
+    p, mx, grid = (dims.enc_patch, dims.enc_pos_max, "encoder") if encode else (dims.dit_patch, dims.dit_pos_max, "decoder")
+    top = 8 * p * mx
+    if H <= 0 or W <= 0 or H % unit or W % unit or H > top or W > top:
+        raise SelftokError(f"image size {H} x {W}: both sides must be positive multiples of {unit} and at most {top} "
+                           f"(the {grid}'s {mx} x {mx} positional grid of {p} x {p} latent patches)")
+    return H // 8, W // 8
 
 
 def _decoder_state(state_dict: Dict, ema_decoder: bool) -> Dict[str, torch.Tensor]:
@@ -258,28 +276,39 @@ class SelftokPipeline:
     # ------------------------------------------------------------------ latent-boundary API (the measured path)
     @torch.no_grad()
     def encode_latents(self, x_0: torch.Tensor) -> torch.Tensor:
-        """x_0 = SD3LatentFormat().process_in(vae.encode(images).mode()).float() -> tokens [B,K] int64 (device)."""
-        return self.engine.encode(x_0)
+        """x_0 = SD3LatentFormat().process_in(vae.encode(images).mode()).float() -> tokens [B,K] int64 (device).  Any latent size
+        within the encoder's positional grid (`latent_size`); the tokens are [B,K] at every size."""
+        hw = tuple(x_0.shape[2:]) if x_0.dim() == 4 else None
+        return self.engine.encode(x_0, latent_hw=hw)
+
+    def _latent_hw(self, size, noise: Optional[torch.Tensor]) -> Tuple[int, int]:
+        hw = latent_size(self.datasize if size is None else size, self.dims)
+        if noise is not None and (noise.dim() != 4 or tuple(noise.shape[2:]) != hw):
+            raise SelftokError(f"noise of shape {tuple(noise.shape)} disagrees with the image size {8 * hw[0]} x {8 * hw[1]} "
+                               f"(latent {hw[0]} x {hw[1]})")
+        return hw
 
     @torch.no_grad()
     def decode_latents(self, idx, noise: Optional[torch.Tensor] = None, cfg_scale: Optional[float] = None, *,
-                       token_range=None) -> torch.Tensor:
+                       token_range=None, size=None) -> torch.Tensor:
         """tokens -> pred_x0 latents after the 50-step Euler loop.  `noise` defaults to the reference's draw:
         torch.randn on the CPU global generator, then moved to the device (SelftokPipeline.py:262-264).
         cfg_scale (None / 1: plain sampler): classifier-free guidance as RectifiedFlow.sample_one_step implements it
         (rectified_flow.py:280-289) -- an explicit argument here because the reference pipeline never forwards its own.
         token_range: decode image b from its ids [lo_b, hi_b) only -- a (lo, hi) pair for the batch or an int array [B, 2]; the
         ids outside the window are not read (pad with anything).  AR models emit the sequence in reverse index order, so n
-        generated tokens = `(K - n, K)`; a truncated prefix is `(0, n)`.  Token rows stay [B, K]."""
+        generated tokens = `(K - n, K)`; a truncated prefix is `(0, n)`.  Token rows stay [B, K].
+        size: the image size to decode at -- an int or (H, W) in pixels, see `latent_size`; default `datasize`.  It sets the
+        latent shape of the noise draw; a given `noise` must have that shape."""
         token_idx = torch.from_numpy(idx) if isinstance(idx, np.ndarray) else idx
         B = token_idx.shape[0]
-        latent_dim = self.datasize // 8
+        hw = self._latent_hw(size, noise)
         if noise is None:
-            noise = torch.randn(B, self.dims.in_channels, latent_dim, latent_dim)
+            noise = torch.randn(B, self.dims.in_channels, *hw)
         if cfg_scale is None or float(cfg_scale) == 1.0:
-            out = self.engine.decode(token_idx, noise, token_range=token_range)
+            out = self.engine.decode(token_idx, noise, token_range=token_range, latent_hw=hw)
         else:
-            out = self.engine.decode_cfg(token_idx, noise, float(cfg_scale), token_range=token_range)
+            out = self.engine.decode_cfg(token_idx, noise, float(cfg_scale), token_range=token_range, latent_hw=hw)
         self._raise_on_bad_ids(token_idx)
         return out
 
@@ -332,7 +361,12 @@ class SelftokPipeline:
             raise SelftokError("no VAE: pass sd3_path (diffusers AutoencoderKL) or vae=..., or use the *_latents methods")
 
     def encoding(self, images, device):
+        """images [B,3,H,W] in [-1,1] of any size `latent_size(..., encode=True)` accepts (the reference's encoding takes any size
+        its encoder's positional grid holds) -> tokens [B,K]."""
         print("Begin encoding.")
+        if images.dim() != 4:
+            raise SelftokError(f"encoding: expected images [B,3,H,W], got {tuple(images.shape)}")
+        latent_size(tuple(images.shape[2:]), self.dims, encode=True)
         self._need_vae()
         images = images.to(dtype=self.dtype, device=device)
         x_0 = self.vae.encode(images, return_dict=False)[0].mode()
@@ -343,11 +377,11 @@ class SelftokPipeline:
         return tokens
 
     @torch.no_grad()
-    def decoding(self, idx, device, *, token_range=None):
-        """token_range: see `decode_latents` (n generated tokens = `(K - n, K)`)."""
+    def decoding(self, idx, device, *, token_range=None, size=None):
+        """token_range, size: see `decode_latents` (n generated tokens = `(K - n, K)`)."""
         print("Begin decoding.")
         self._need_vae()
-        pred_x0 = self.decode_latents(idx, token_range=token_range)
+        pred_x0 = self.decode_latents(idx, token_range=token_range, size=size)
         recons = self._latents_to_pixels(pred_x0)
         print("End decoding.")
         return recons
@@ -367,10 +401,11 @@ class SelftokPipeline:
         return ContinuousDecoder(self.engine, max_batch, guided=guided, postprocess=torch.no_grad()(self._latents_to_pixels))
 
     @torch.no_grad()
-    def decoding_cfg(self, idx, device, cfg_scale: Optional[float] = None, *, token_range=None):
-        """decoding() with the guided sampler (cfg_scale defaults to the constructor's); token_range as in `decode_latents`."""
+    def decoding_cfg(self, idx, device, cfg_scale: Optional[float] = None, *, token_range=None, size=None):
+        """decoding() with the guided sampler (cfg_scale defaults to the constructor's); token_range and size as in `decode_latents`."""
         self._need_vae()
-        pred_x0 = self.decode_latents(idx, cfg_scale=self.cfg_scale if cfg_scale is None else cfg_scale, token_range=token_range)
+        pred_x0 = self.decode_latents(idx, cfg_scale=self.cfg_scale if cfg_scale is None else cfg_scale, token_range=token_range,
+                                      size=size)
         return self._latents_to_pixels(pred_x0)
 
     @torch.no_grad()
